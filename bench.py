@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline metric of BASELINE.json: basecalled samples/s on B200.
+"""bench.py -- headline metric: basecalled samples/s on one H100 (sm_90a).
 
 One "step" = one pass of the hot path (network forward + CRF decode) over one batch of synthetic chunks.
 Workload at N=1: BASELINE.json configs[1] -- dna_r10.4.1 fast@v5 topology, batch 512, chunksize 10000
@@ -27,6 +27,13 @@ embarrassingly; no collective on the data path) -> weak scaling; time = max over
 
 `--impl reference` times only the CPU runner: a step is one pass of every runner over its 4 chunks; W warm-up passes,
 then exactly K timed passes, value = samples of the K passes / their wall time.
+
+`--steps K` is the number of timed steps of every timed region (also of the hac / sup sub-results of the default run).
+`--dump-outputs DIR` writes, after the timed steps, what the last timed call of each runner on the END-TO-END path (`e2e`:
+b200_runner_call_chunks from host buffers) returned -- moves, sequence, qstring [batch, T_out] and n_bases [batch] -- as
+DIR/runner<i>_<name>.npy in float32.  The device-resident path behind `value` runs the same forward + decode on the same
+batches but its results are never read back.  Inputs and weights are seeded, so two builds run with the same arguments can
+be compared array for array.
 """
 from __future__ import annotations
 
@@ -51,8 +58,8 @@ MODELS = {
 }
 # SURVEY.md section 8(d): algorithmic FLOP per input sample
 FLOP_PER_SAMPLE = {"fast": 0.1435e6, "hac": 2.139e6, "sup": 14.35e6}
-SUB_MODELS = {"hac": dict(batch=512, steps=8), "sup": dict(batch=128, steps=6)}
-NUM_SMS = 148
+SUB_MODELS = {"hac": dict(batch=512), "sup": dict(batch=128)}
+NUM_SMS = 132   # H100 SXM
 DEFAULT_RUNNERS = {"fast": 4, "hac": 4, "sup": 2}   # batches in flight per GPU (dorado's --num-runners; see --runners)
 METRIC = "basecalled samples/s"
 
@@ -67,7 +74,8 @@ def peaks():
         d = json.loads(p.read_text())
         return dict(hbm_gbs=d["hbm_gbs"], tflops=d["bf16_tflops"], tflops_sustained=d.get("bf16_tflops_sustained"),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, tflops=1590.0, tflops_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W card): HBM3 3.35 TB/s, dense FP16 989 TFLOP/s; not a measured peak
+    return dict(hbm_gbs=3350.0, tflops=989.0, tflops_sustained=None, source="H100 SXM data sheet (dense fp16)")
 
 
 class ClockSampler:
@@ -254,10 +262,10 @@ def cpu_baseline_leg(kind, chunksize):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ---------------------------------------------------------------------------------------------------------------------
 def kernel_work(cfg, kind, N, T, T_out):
-    """Algorithmic work of ONE launch of each kernel (SURVEY.md 8d; DESIGN.md section 4): name -> (bound, amount)."""
+    """Algorithmic work of ONE launch of each kernel (SURVEY.md 8d): name -> (bound, amount)."""
     C = cfg.outsize
     S = C // 4
     if cfg.is_tx_model:
@@ -285,7 +293,30 @@ def kernel_work(cfg, kind, N, T, T_out):
     return work
 
 
-def bench_b200(kind, batch, chunksize, steps, warmup, R, rank, local_rank, world, sampler=None, want_cpu=False):
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(directory, results):
+    """results: one (moves, seq, qstring, n_bases) per runner -> DIR/runner<i>_<name>.npy (float32).  Above 64 MB in all,
+    the same seeded sample of chunks (rows) is kept from every array."""
+    out = pathlib.Path(directory)
+    out.mkdir(parents=True, exist_ok=True)
+    arrays = {}
+    for i, res in enumerate(results):
+        for name, a in zip(("moves", "sequence", "qstring", "n_bases"), res):
+            arrays[f"runner{i}_{name}"] = np.asarray(a, np.float32)
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT_BYTES:
+        rows = arrays["runner0_moves"].shape[0]
+        keep = max(1, int(rows * DUMP_LIMIT_BYTES / total))
+        idx = np.sort(np.random.default_rng(0).choice(rows, size=keep, replace=False))
+        arrays = {k: a[idx] for k, a in arrays.items()}
+    for k, a in arrays.items():
+        np.save(out / f"{k}.npy", a)
+
+
+def bench_b200(kind, batch, chunksize, steps, warmup, R, rank, local_rank, world, sampler=None, want_cpu=False,
+               dump_dir=None):
     import torch
     import torch.distributed as dist
     from dorado_b200.config import load_model_config
@@ -354,6 +385,8 @@ def bench_b200(kind, batch, chunksize, steps, warmup, R, rank, local_rank, world
     run_calls(steps)
     barrier()
     e2e_s = max_over_ranks(time.perf_counter() - t0)
+    if dump_dir is not None and rank == 0:
+        dump_outputs(dump_dir, [tuple(np.array(a) for a in res) for res in last if res is not None])
     bases_last = int(next(c for c in last if c is not None)[3][:N].sum())
     e2e_value = world * samples_per_step * steps / e2e_s
     h2d = N * T * 2
@@ -419,20 +452,6 @@ def bench_b200(kind, batch, chunksize, steps, warmup, R, rank, local_rank, world
     roof["decode"] = {"bound": "hbm", "algorithmic_bytes": dec_alg, "ms": round(dec_total_ms, 4),
                       "achieved": round(dec_alg / (dec_total_ms * 1e-3) / 1e9, 2),
                       "frac": round(dec_alg / (dec_total_ms * 1e-3) / 1e9 / pk["hbm_gbs"], 4)}
-    # DRAM bytes per launch from this round's `ncu --set full` captures of the same workload (profiles/r02_traffic.json,
-    # written by tools/ncu_summary.py): for the dominant kernel as roofline.traffic, and per kernel; null when not captured
-    try:
-        tr_all = json.loads((ROOT / "profiles" / "r02_traffic.json").read_text())
-    except (OSError, ValueError):
-        tr_all = {}
-    for k, e in roof["per_kernel"].items():
-        tr = tr_all.get(f"{kind}_n{N}_{k}")
-        if tr:
-            e["traffic"] = tr["dram_bytes"]
-    tr = tr_all.get(f"{kind}_n{N}_{dom}")
-    if tr:
-        roof["traffic"] = tr["dram_bytes"]
-        roof["traffic_source"] = f"profiles/{tr['file']} launch {tr['launch']} ({tr['kernel']})"
     roof["peak_source"] = pk["source"]
     roof["ms_per_launch"] = dom_ms
     roof["launches_per_step"] = dom_cnt
@@ -465,9 +484,11 @@ def main():
     ap.add_argument("--runners", type=int, default=None,
                     help="runners (batches in flight) per GPU = dorado's --num-runners (default there 2 per device, "
                          "api/runner_creation.cpp:91-123).  Default here: 4 for fast (its recurrence and beam search are latency "
-                         "chains; four batches side by side fill the SMs, profiles/r02_b11_*), 2 for hac and sup")
+                         "chains; four batches side by side fill the SMs), 2 for hac and sup")
     ap.add_argument("--no-cpu-baseline", action="store_true", help="skip the CPU reference leg (batch sweeps)")
     ap.add_argument("--no-sub-models", action="store_true", help="skip the hac@512 / sup@128 sub-results of the default run")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last end-to-end call's outputs of every runner as DIR/*.npy")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -482,7 +503,7 @@ def main():
                           f"{args.chunksize} -> {T} samples/chunk, synthetic N(0,1) fp16 signal",
               "model": kind, "batch_per_gpu": args.batch, "chunk_samples": T, "parallelism": f"replica x{args.gpus}",
               "runners_per_gpu": args.runners if args.runners is not None else DEFAULT_RUNNERS[kind],
-              "l2": "per-step working set (conv activations + scores > 400 MB) exceeds the 126 MB L2; no explicit flush"}
+              "l2": "per-step working set (conv activations + scores > 400 MB) exceeds the 50 MB L2; no explicit flush"}
 
     if args.impl == "reference":
         if rank != 0:
@@ -493,7 +514,7 @@ def main():
     import torch
     import torch.distributed as dist
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device; the B200 engine has no CPU fallback")
+        raise SystemExit("bench.py: no CUDA device; the engine has no CPU fallback")
     torch.cuda.set_device(local_rank)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
@@ -504,12 +525,12 @@ def main():
     R = max(1, args.runners if args.runners is not None else DEFAULT_RUNNERS[kind])
     config["runners_per_gpu"] = R
     main_res = bench_b200(kind, args.batch, args.chunksize, args.steps, args.warmup, R, rank, local_rank, world, sampler=sampler,
-                          want_cpu=(world == 1 and not args.no_cpu_baseline))
+                          want_cpu=(world == 1 and not args.no_cpu_baseline), dump_dir=args.dump_outputs)
     subs = {}
     default_run = kind == "fast" and args.batch == 512 and not args.no_sub_models
     if default_run:
         for sk, sc in SUB_MODELS.items():
-            res = bench_b200(sk, sc["batch"], args.chunksize, sc["steps"], 3, DEFAULT_RUNNERS[sk], rank, local_rank, world)
+            res = bench_b200(sk, sc["batch"], args.chunksize, args.steps, 3, DEFAULT_RUNNERS[sk], rank, local_rank, world)
             if rank == 0:
                 keep = ("value", "ms_per_step", "steps", "e2e", "forward_ms_per_step", "decode_ms_per_step", "batch_per_gpu",
                         "chunk_samples", "runners_per_gpu", "gpu_launches", "bases_called_last_step")
@@ -518,7 +539,7 @@ def main():
                 subs[sk]["roofline"] = {k: r[k] for k in ("kernel", "bound", "achieved", "peak", "unit", "frac", "share_of_step",
                                                           "per_kernel", "decode", "forward_tflops", "traffic")}
         # BASELINE.json configs[2], [3]: the same models at the batch size the engine picks itself -- the counterpart of
-        # CudaCaller::determine_batch_dims (pre-computed "NVIDIA B200" table + exact memory cap at 80 % of the free HBM)
+        # CudaCaller::determine_batch_dims (pre-computed timing table + exact memory cap at 80 % of the free HBM)
         from dorado_b200 import batching
         from dorado_b200.config import load_model_config as _lc
         from dorado_b200.runner import B200Caller
@@ -531,7 +552,7 @@ def main():
                                                          num_runners=DEFAULT_RUNNERS[sk])
             probe.close()
             auto_batch = int(dims[0][0])
-            res = bench_b200(sk, auto_batch, args.chunksize, max(3, sc["steps"] // 2), 3, DEFAULT_RUNNERS[sk], rank, local_rank, world)
+            res = bench_b200(sk, auto_batch, args.chunksize, args.steps, 3, DEFAULT_RUNNERS[sk], rank, local_rank, world)
             if rank == 0:
                 subs[sk + "_auto_batch"] = {k: res[k] for k in ("value", "ms_per_step", "steps", "e2e", "batch_per_gpu",
                                                                "chunk_samples", "runners_per_gpu", "gpu_launches")}

@@ -40,7 +40,7 @@ int guarded(F&& fn) {
 extern "C" {
 
 const char* b200_last_error(void) { return g_last_error.c_str(); }
-const char* b200_version(void) { return "b200call 0.1 (sm_100a)"; }
+const char* b200_version(void) { return "b200call 0.1 (sm_90a)"; }
 
 int b200_device_count(void) {
     int n = 0;

@@ -1,9 +1,9 @@
-// Pre-computed batch-size timings: the B200 counterpart of CudaChunkBenchmarks
+// Pre-computed batch-size timings: the counterpart of CudaChunkBenchmarks
 // (dorado/basecall/benchmarks/CudaChunkBenchmarks.cpp:14-77 and the per-GPU tables next to it).  determine_batch_dims
 // (CudaCaller.cpp:506-557) looks the (GPU name, model name) pair up before it falls back to timing every batch size at
-// start-up.  The table below was measured on this engine by tools/gen_chunk_benchmarks.py on an NVIDIA B200 (forward +
-// decode of one batch at the full chunk size, ms per chunk, only the batch sizes that improve on every smaller one, as the
-// reference's generator keeps them).
+// start-up.  Tables are produced on the GPU by tools/gen_chunk_benchmarks.py (forward + decode of one batch at the full
+// chunk size, ms per chunk, only the batch sizes that improve on every smaller one, as the reference's generator keeps
+// them); chunk_benchmarks_b200.inc holds what has been measured for this engine.
 #include "engine.h"
 
 #include <cstring>
@@ -28,7 +28,7 @@ struct Table {
 
 // GPUs that share a table (CudaChunkBenchmarks.cpp:39-46 keeps the same kind of alias list)
 const char* canonical_gpu(const std::string& name) {
-    if (name == "NVIDIA B200" || name == "NVIDIA B200 SXM" || name == "NVIDIA HGX B200") return "NVIDIA B200";
+    if (name == "NVIDIA H100 80GB HBM3" || name == "NVIDIA H100 SXM5 80GB" || name == "NVIDIA H100") return "NVIDIA H100 80GB HBM3";
     return nullptr;
 }
 
@@ -38,7 +38,8 @@ int lookup_chunk_benchmarks(const char* gpu_name, const char* model_name, int32_
     if (!gpu_name || !model_name) throw std::invalid_argument("chunk benchmarks: null name");
     const char* gpu = canonical_gpu(gpu_name);
     if (!gpu) return 0;
-    for (const Table& t : kTables) {
+    for (int k = 0; k < kNumTables; ++k) {
+        const Table& t = kTables[k];
         if (std::strcmp(t.gpu, gpu) == 0 && std::strcmp(t.model, model_name) == 0) {
             for (int i = 0; i < t.count && i < capacity; ++i) {
                 if (batch_sizes) batch_sizes[i] = t.rows[i].batch_size;

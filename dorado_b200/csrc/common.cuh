@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels of the B200 basecalling engine.
+// Shared helpers for the sm_90a kernels of the basecalling engine.
 #pragma once
 
 #include <cuda_fp16.h>
@@ -21,7 +21,7 @@ inline void cuda_check(cudaError_t e, const char* what, const char* file, int li
 }
 #define B200_CUDA(expr) ::b200::cuda_check((expr), #expr, __FILE__, __LINE__)
 
-constexpr int kNumSMs = 148;
+constexpr int kNumSMs = 132;   // H100 SXM
 
 // exact warp-wide max of finite floats in one redux.sync: order-preserving float <-> uint32 key
 __device__ __forceinline__ float warp_max(float v) {

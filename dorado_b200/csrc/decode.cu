@@ -1,4 +1,4 @@
-// CRF decode for sm_100a: backward scan -> fused forward scan / posteriors / beam search -> traceback.
+// CRF decode for sm_90a: backward scan -> fused forward scan / posteriors / beam search -> traceback.
 //
 // Replaces the closed Koi kernels behind dorado/basecall/decode/CUDADecoder.cpp:76-104
 // (host_back_guide_step, host_beam_search_step, host_compute_posts_step, host_run_decode) and the CPU
@@ -274,10 +274,9 @@ __device__ __forceinline__ float kmer_block_prob(const float* post_row, int stat
 // One block of the beam search for one chunk, executed by one warp (lane = beam element).
 // Returns the new beam width; writes the kept elements (meta plane) and their block probabilities (prob plane).
 //
-// Measured on the B200 (profiles/r02_b17_*): the decode kernels are bound by instruction issue -- the backward scan runs at
-// ~0.5 instructions per cycle and scheduler on the SMs it occupies, and the beam warp's block time is its instruction count
-// times ~3 cycles -- so the step is written for few instructions: an in-kernel experiment that evaluated three levels of the
-// beam-cut bisection at once (7 cutoffs per round) shortened the dependent chain and made the kernel SLOWER.
+// The decode kernels are bound by instruction issue -- the beam warp's block time is its instruction count times a few
+// cycles -- so the step is written for few instructions: evaluating three levels of the beam-cut bisection at once
+// (7 cutoffs per round) shortens the dependent chain but costs more instructions than it saves.
 //   * stay/step merge: a stay i can only merge with the step (j, b_i) whose previous hash is crc2_inv(hash_i, b_i); that j is
 //     found through a 1024-entry lane-id table over the low hash bits (one byte store, one byte load, one compare) instead of
 //     comparing against all 32 hashes.  Lanes whose table entry was overwritten by another lane (a slot shared by two

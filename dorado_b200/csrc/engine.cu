@@ -82,7 +82,7 @@ float log_beam_cut_of(float beam_cut) {
     return beam_cut > 0.0f ? logf(beam_cut) : std::numeric_limits<float>::max();
 }
 
-void require_sm100(int device) {
+void require_sm90(int device) {
     int count = 0;
     if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) {
         cudaGetLastError();
@@ -91,9 +91,9 @@ void require_sm100(int device) {
     if (device < 0 || device >= count) throw std::invalid_argument("b200call: bad device index");
     cudaDeviceProp prop{};
     B200_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) {
+    if (prop.major != 9 || prop.minor != 0) {
         throw CudaError(std::string("b200call: device '") + prop.name + "' is sm_" + std::to_string(prop.major) +
-                        std::to_string(prop.minor) + "; this build contains sm_100a code only");
+                        std::to_string(prop.minor) + "; this build contains sm_90a code only");
     }
     B200_CUDA(cudaSetDevice(device));
 }
@@ -104,7 +104,7 @@ Engine::Engine(const b200_model_desc& desc, const b200_tensor* tensors, int num_
     if (desc.outsize != (1 << (2 * (desc.state_len + 1)))) throw std::invalid_argument("outsize != 4^(state_len+1)");
     if (desc.num_convs < 1 || desc.num_convs > 8) throw std::invalid_argument("num_convs must be in [1, 8]");
     if (desc.stride < 1) throw std::invalid_argument("stride must be positive");
-    require_sm100(device);
+    require_sm90(device);
     B200_CUDA(cudaStreamCreateWithFlags(&m_stream, cudaStreamNonBlocking));
     if (desc.model_type == B200_MODEL_LSTM) {
         m_model = make_lstm_model(desc, tensors, num_tensors);
@@ -705,7 +705,7 @@ void decode_host_scores(int device, const uint16_t* scores, int N, int T, int C,
     if (!state_len) throw std::invalid_argument("decode: C must be 4^(state_len+1) with state_len 3..5");
     if (opts.move_pad != 0) throw Unsupported("move_pad: only the closed Koi kernel defines it; the reference never sets it");
     if (opts.temperature != 1.0f) throw Unsupported("temperature != 1: no decoder of the reference reads this option");
-    require_sm100(device);
+    require_sm90(device);
     cudaStream_t s;
     B200_CUDA(cudaStreamCreate(&s));
     size_t bwd_b = 0, beam_b = 0;

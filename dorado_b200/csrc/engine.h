@@ -286,6 +286,6 @@ inline void ensure_dynamic_smem(K* kernel, int bytes) {
 }
 
 float log_beam_cut_of(float beam_cut);
-void require_sm100(int device);
+void require_sm90(int device);
 
 }  // namespace b200

@@ -1,16 +1,16 @@
-// tcgen05 GEMM for the dense layers of the basecaller (last conv as a strided GEMM, CRF linear, and every
-// transformer projection).  Successor of the reference's cuBLAS/Koi call sites:
+// wgmma GEMM for the dense layers of the basecaller (last conv as a strided GEMM, CRF linear, LSTM input projection and
+// every transformer projection).  Successor of the reference's cuBLAS/Koi call sites:
 //   matmul_f16 (cublasGemmEx)      dorado/torch_utils/cuda_utils.cpp:386-403
 //   host_linear / cutlass conv     dorado/nn/ConvStack.cpp:257, dorado/nn/CRFModules.cpp:112
 //   koi_linear / koi_mm_swiglu     dorado/nn/TxModules.cpp:653-697
 //
-// Persistent: one CTA per SM loops over 128 x BN output tiles.  Warp roles: warp 0 = TMA producer (A and W tiles,
-// 128-byte swizzle, 4-stage mbarrier ring that runs across tiles), warp 1 = single-thread tcgen05.mma issuer,
-// warps 2-9 = epilogue (tcgen05.ld -> bias / activation / residual -> fp16 -> 16-byte global stores).  The
-// accumulator is double-buffered in TMEM (2 x BN columns) so the epilogue of tile i overlaps the MMAs of tile i+1.
-// A is addressed through a 3-D tensor map (k, row, batch) so that overlapping-row views work: the last
-// conv of the LSTM models reads its im2col rows straight from the NTC activation buffer with row stride
-// = stride * C_in (the reference's "cutlass_conv" trick, ConvStack.cpp:236-275).
+// Persistent: one CTA per SM loops over 128 x BN output tiles (BN <= 128).  Warpgroup 0 is the TMA producer (one thread:
+// A and W tiles, 128-byte swizzle, a STAGES-deep mbarrier ring that runs across tiles); warpgroups 1 and 2 own rows 0-63 and
+// 64-127 of the tile: they issue wgmma m64n32k16 straight from the swizzled stages, keep the fp32 accumulator in registers
+// and run the epilogue (bias / activation / residual / rotary / SwiGLU -> fp16 -> global) from the accumulator fragments.
+// A is addressed through a 3-D tensor map (k, row, batch) so that overlapping-row views work: the last conv of the LSTM
+// models reads its im2col rows straight from the NTC activation buffer with row stride = stride * C_in (the reference's
+// "cutlass_conv" trick, ConvStack.cpp:236-275).
 #include "gemm.h"
 
 #include "common.cuh"
@@ -26,42 +26,26 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int STAGES = 4;  // default ring depth
-constexpr int GEMM_PARTS = 4;                        // column parts of a tile, each drained by one set of 4 epilogue warps
-constexpr int GEMM_EPI_WARPS = 4 * GEMM_PARTS;       // a set = one warp per TMEM lane quarter
-constexpr int GEMM_THREADS = 64 + 32 * GEMM_EPI_WARPS;
-
-// 32-column chunks [cb, ce) of a tile of nch chunks that part `part` drains.  `unit` = chunks that must stay together (2 for
-// the rotary epilogue: x1 | x2 of a head).  Parts beyond the number of units get nothing.
-__host__ __device__ inline void gemm_part_range(int nch, int unit, int part, int* cb, int* ce) {
-    const int units = nch / unit;
-    const int nparts = units < GEMM_PARTS ? units : GEMM_PARTS;
-    if (part >= nparts) {
-        *cb = *ce = nch;
-        return;
-    }
-    *cb = (part * units / nparts) * unit;
-    *ce = ((part + 1) * units / nparts) * unit;
-}
+constexpr int BN_MAX = 128;
+constexpr int STAGES = 5;          // TMA -> wgmma ring depth: 5 x 32 KB of the 227 KB
+constexpr int GEMM_PARTS = 4;      // RMSNorm partial sums per row and column tile (GemmDesc::out_ss): one per 32-column chunk
+constexpr int GEMM_THREADS = 384;  // warpgroup 0: producer; warpgroups 1, 2: MMA + epilogue of 64 rows each
 
 struct GemmKernelParams {
-    int rows_per_batch, tiles_per_batch, N, num_k_blocks, bn, act;
-    int num_tiles, n_tiles;  // total tiles, tiles along N
+    int rows_per_batch, tiles_per_batch, N, num_k_blocks, bn;
+    int num_tiles, n_tiles, m_tiles;  // total tiles, tiles along N, row tiles (all batches)
+    int mfast;                        // row tile index runs fastest (fewer row tiles than column tiles)
     const float* bias;
     __half* out;
-    long long out_m1, out_s0, out_s1;
-    long long out_col_m1, out_col_s0;
+    uint32_t out_m1;
+    long long out_s0, out_s1;
+    uint32_t out_col_m1;
+    long long out_col_s0;
     int bias_per_row;
     const float* rope;
     int rope_T, rope_cols, rope_stride;
     const __half* residual;
     float alpha;
-    uint32_t tmem_cols;
-    // staged epilogue: the fp16 tile goes through swizzled shared memory and leaves as TMA stores (tma_o)
-    int staged;      // 0 = per-thread global stores
-    int res_tma;     // staged only: the residual tile is TMA-loaded into the staging tile before the epilogue reads it
-    int stages;      // TMA->MMA ring depth (3 when the staging tile needs the room)
-    int sw;          // columns of a staging sub-tile: 64 (128-byte swizzle) or 32 (64-byte swizzle)
     // RMSNorm folded into the epilogue (GemmDesc)
     float* out_ss;
     const float* a_ss;
@@ -69,34 +53,12 @@ struct GemmKernelParams {
     const float* res_gain;
     int a_ss_parts, res_ss_parts;
     float norm_inv_dim, norm_eps;
-    int out_kind;    // coordinates of a sub-tile: 0 (col, row, batch)  1 (col, g % out_P, g / out_P)  2 (0, row, col / 32)
-    int out_P;
-    // operand-stationary schedules.  wstat = 1: CTA b owns column tile b % n_tiles for its whole life, keeps that slice of W (all
-    // num_k_blocks K blocks) resident in shared memory and walks the row tiles b / n_tiles, + gridDim.x / n_tiles, ...
-    // wstat = 2: the same with the roles swapped -- row tile b % m_tiles of A resident, column tiles streamed.
-    int wstat;
-    int m_tiles;     // row tiles (all batches)
-    int mfast;       // default schedule: row tile index runs fastest (fewer row tiles than column tiles)
 };
 
-// i-th tile of this CTA: row tile mt, column tile nt; false when the CTA has run out of tiles.  All three roles walk the same
-// sequence.
+// i-th tile of this CTA: row tile mt, column tile nt; false when the CTA has run out of tiles.  Producer and consumers walk
+// the same sequence.  CTAs take consecutive tiles, and the SHORTER dimension runs fastest, so that the CTAs working at any
+// moment share their tiles of the long operand (read from HBM once, then served by L2) and sweep the long operand once.
 __device__ __forceinline__ bool gemm_tile_at(const GemmKernelParams& p, int i, int* mt, int* nt) {
-    if (p.wstat == 1) {
-        *nt = (int)blockIdx.x % p.n_tiles;
-        *mt = (int)blockIdx.x / p.n_tiles + i * ((int)gridDim.x / p.n_tiles);
-        return *mt < p.m_tiles;
-    }
-    if (p.wstat == 2) {
-        *mt = (int)blockIdx.x % p.m_tiles;
-        *nt = (int)blockIdx.x / p.m_tiles + i * ((int)gridDim.x / p.m_tiles);
-        return *nt < p.n_tiles;
-    }
-    // default schedule: CTAs take consecutive tiles, and the SHORTER dimension runs fastest, so that the CTAs working at any
-    // moment share their tiles of the long operand (read from HBM once, then served by L2) and sweep the long operand once.
-    // With the column tile always fastest, the hac x-projection (12 row tiles of W_ih against 3332 column tiles of
-    // activations) swept the 655 MB of activations once per row tile: 7.9 GB of DRAM reads per launch, 81 % of the HBM
-    // peak (profiles/r02_gx_gemm_hac_n512.raw.csv).
     const int tile = (int)blockIdx.x + i * (int)gridDim.x;
     if (p.mfast) {
         *mt = tile % p.m_tiles;
@@ -108,10 +70,8 @@ __device__ __forceinline__ bool gemm_tile_at(const GemmKernelParams& p, int i, i
     return tile < p.num_tiles;
 }
 
-constexpr int kMaxStages = 4;
-
 // The activation is a template parameter of the kernel: with a run-time switch inside the unrolled epilogue loops the
-// compiler if-converts it and every element pays for every variant's ex2 / rcp (measured: 2.7x on the plain-store GEMMs).
+// compiler if-converts it and every element pays for every variant's ex2 / rcp.
 template <int ACT>
 __device__ __forceinline__ float act_apply(float v) {
     if constexpr (ACT == GEMM_ACT_SWISH) return swish_fast(v);
@@ -121,385 +81,222 @@ __device__ __forceinline__ float act_apply(float v) {
     else return v;
 }
 
+// One K block (64) of a warpgroup's 64 x 32 NCH tile: 32 rows of W are 4 KB further on, 16 fp16 along K are +2 in the
+// (addr >> 4) field of a descriptor.
+template <int NCH>
+__device__ __forceinline__ void wgmma_k_block(float (&acc)[BN_MAX / 32][16], uint64_t adesc, uint64_t bdesc, bool accumulate) {
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) {
+#pragma unroll
+        for (int c = 0; c < NCH; ++c) {
+            tc::wgmma_m64n32k16(acc[c], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(c * 256 + 2 * k), accumulate || k != 0);
+        }
+    }
+}
+
 template <int ACT>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_tcgen05_kernel(const __grid_constant__ CUtensorMap tma_a,
-                                                                           const __grid_constant__ CUtensorMap tma_w,
-                                                                           const __grid_constant__ CUtensorMap tma_o,
-                                                                           const __grid_constant__ CUtensorMap tma_r,
-                                                                           const GemmKernelParams p) {
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a,
+                                                                         const __grid_constant__ CUtensorMap tma_w,
+                                                                         const GemmKernelParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // carve: stages x (A 16 KB | W bn*128 B), then barriers
     // realign by an integer offset from the __shared__ symbol so the compiler keeps the shared address space
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
     const uint32_t a_bytes = BM * BK * 2;
-    const uint32_t w_bytes = (uint32_t)p.bn * BK * 2;
-    // ring stage: A | W, or only the streamed operand when the other one is resident (its K blocks sit in front of the ring)
-    const uint32_t res_kb_bytes = p.wstat == 1 ? w_bytes : a_bytes;   // one K block of the resident operand
-    const uint32_t stage_bytes = p.wstat == 0 ? a_bytes + w_bytes : (p.wstat == 1 ? a_bytes : w_bytes);
-    const int NST = p.stages;
-    uint8_t* w_res = smem;
-    uint8_t* ring = smem + (p.wstat ? (uint32_t)p.num_k_blocks * res_kb_bytes : 0u);
-    // staging tile of the epilogue: two column halves (one per epilogue warp set), 128 rows x bn/2 fp16 each
-    uint8_t* stage_out = ring + NST * stage_bytes;
-    // staging tile: [128 rows][bn output columns] fp16 as sub-tiles of p.sw columns, partitioned by column range among the parts
-    const uint32_t staging_bytes = p.staged ? (uint32_t)(BM * (p.bn / (ACT == GEMM_ACT_SWIGLU ? 2 : 1)) * 2) : 0u;
-    uint64_t* full = reinterpret_cast<uint64_t*>(stage_out + staging_bytes);
-    uint64_t* empty = full + kMaxStages;
-    uint64_t* tmem_full = empty + kMaxStages;   // [2]
-    uint64_t* tmem_empty = tmem_full + 2;   // [2]
-    uint64_t* res_full = tmem_empty + 2;    // [GEMM_PARTS] residual tile landed in the part's staging columns
-    uint64_t* w_full = res_full + GEMM_PARTS;   // weight-stationary: the resident W slice has landed
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(w_full + 1);
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
+    const uint32_t w_bytes = (uint32_t)p.bn * BK * 2;   // a multiple of 4 KB: every stage stays 1024-byte aligned
+    const uint32_t stage_bytes = a_bytes + w_bytes;
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * stage_bytes);
+    uint64_t* empty = full + STAGES;
+    const int nch = p.bn / 32;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < NST; ++s) {
+        for (int s = 0; s < STAGES; ++s) {
             tc::mbar_init(&full[s], 1);
-            tc::mbar_init(&empty[s], 1);
+            tc::mbar_init(&empty[s], 2);   // one arrival per consumer warpgroup
         }
-        for (int i = 0; i < 2; ++i) {
-            tc::mbar_init(&tmem_full[i], 1);
-            tc::mbar_init(&tmem_empty[i], 32 * GEMM_EPI_WARPS);
-        }
-        for (int i = 0; i < GEMM_PARTS; ++i) tc::mbar_init(&res_full[i], 1);
-        tc::mbar_init(w_full, 1);
         tc::fence_barrier_init();
         tc::prefetch_tmap(&tma_a);
         tc::prefetch_tmap(&tma_w);
-        if (p.staged) tc::prefetch_tmap(&tma_o);
-        if (p.res_tma) tc::prefetch_tmap(&tma_r);
     }
-    if (warp == 1) tc::tmem_alloc(tmem_holder, p.tmem_cols);
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_base = *tmem_holder;
+    const int wg = threadIdx.x >> 7;
 
-    if (warp == 0) {
-        if (tc::elect_one()) {
-            int s = 0;            // ring slot and its phase, advanced incrementally (the ring depth is a run-time value)
-            uint32_t ph = 0;
-            int mt, nt;
-            if (p.wstat && gemm_tile_at(p, 0, &mt, &nt)) {
-                tc::mbar_arrive_expect_tx(w_full, (uint32_t)p.num_k_blocks * res_kb_bytes);
-                for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-                    if (p.wstat == 1) {
-                        tc::tma_load_2d(w_res + (size_t)kb * res_kb_bytes, &tma_w, w_full, kb * BK, nt * p.bn);
-                    } else {
-                        tc::tma_load_3d(w_res + (size_t)kb * res_kb_bytes, &tma_a, w_full, kb * BK, (mt % p.tiles_per_batch) * BM,
-                                        mt / p.tiles_per_batch);
-                    }
-                }
-            }
-            for (int i = 0; gemm_tile_at(p, i, &mt, &nt); ++i) {
-                const int batch = mt / p.tiles_per_batch;
-                const int r0 = (mt % p.tiles_per_batch) * BM;
-                const int n0 = nt * p.bn;
-                for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-                    tc::mbar_wait(&empty[s], ph ^ 1);
-                    tc::mbar_arrive_expect_tx(&full[s], stage_bytes);
-                    uint8_t* a_s = ring + s * stage_bytes;
-                    if (p.wstat != 2) tc::tma_load_3d(a_s, &tma_a, &full[s], kb * BK, r0, batch);
-                    if (p.wstat != 1) tc::tma_load_2d(a_s + (p.wstat == 2 ? 0u : a_bytes), &tma_w, &full[s], kb * BK, n0);
-                    if (++s == NST) {
-                        s = 0;
-                        ph ^= 1;
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (tc::elect_one()) {
-            const uint32_t idesc = tc::umma_idesc_f16(BM, p.bn);
+    if (wg == 0) {
+        if (threadIdx.x == 0) {
             int s = 0;
             uint32_t ph = 0;
             int mt, nt;
-            if (p.wstat && gemm_tile_at(p, 0, &mt, &nt)) {
-                tc::mbar_wait(w_full, 0);
-                tc::tc_fence_after();
-            }
-            for (int ti = 0; gemm_tile_at(p, ti, &mt, &nt); ++ti) {
-                const int ab = ti & 1;
-                tc::mbar_wait(&tmem_empty[ab], (uint32_t)(((ti >> 1) & 1) ^ 1));
-                tc::tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(ab * p.bn);
+            for (int i = 0; gemm_tile_at(p, i, &mt, &nt); ++i) {
+                const int batch = mt / p.tiles_per_batch;
+                const int r0 = (mt % p.tiles_per_batch) * BM;
                 for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-                    tc::mbar_wait(&full[s], ph);
-                    tc::tc_fence_after();
-                    const uint32_t st_addr = tc::smem_u32(ring + s * stage_bytes);
-                    const uint32_t rs_addr = tc::smem_u32(w_res + (size_t)kb * res_kb_bytes);
-                    const uint64_t adesc = tc::umma_desc_sw128(p.wstat == 2 ? rs_addr : st_addr);
-                    const uint64_t bdesc = tc::umma_desc_sw128(p.wstat == 1 ? rs_addr : (p.wstat == 2 ? st_addr : st_addr + a_bytes));
-#pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        // advance 16 fp16 = 32 B along K inside the 128 B swizzle row: +2 in the (addr >> 4) field
-                        tc::umma_f16(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (kb | k) != 0);
-                    }
-                    tc::umma_commit(&empty[s]);
-                    if (++s == NST) {
+                    tc::mbar_wait_silent(&empty[s], ph ^ 1);
+                    tc::mbar_arrive_expect_tx(&full[s], stage_bytes);
+                    uint8_t* st = smem + s * stage_bytes;
+                    tc::tma_load_3d(st, &tma_a, &full[s], kb * BK, r0, batch);
+                    tc::tma_load_2d(st + a_bytes, &tma_w, &full[s], kb * BK, nt * p.bn);
+                    if (++s == STAGES) {
                         s = 0;
                         ph ^= 1;
                     }
                 }
-                tc::umma_commit(&tmem_full[ab]);
             }
         }
-    } else {
-        // epilogue: warp w may only touch TMEM lanes [32 * (w % 4), +32)
-        const int lg = warp & 3;
-        const int part = (warp - 2) >> 2;  // which part of the tile's columns this warp set drains
-        const int nch = p.bn / 32;
-        int c_begin, c_end;
-        gemm_part_range(nch, ACT == GEMM_ACT_ROPE ? 2 : 1, part, &c_begin, &c_end);
-        const int n_out_total = ACT == GEMM_ACT_SWIGLU ? p.N / 2 : p.N;
-        // staged epilogue: this warp set owns the staging columns of its part; thread = tile row
-        const bool staged = p.staged != 0;
-        constexpr int out_div = ACT == GEMM_ACT_SWIGLU ? 2 : 1;            // output columns per accumulator column
-        uint8_t* my_stage = stage_out + (size_t)(c_begin * 32 / out_div) * BM * 2;
-        const int trow = lg * 32 + lane;
-        const bool storer = staged && lg == 0 && lane == 0 && c_begin < c_end;
-        const int bar_free = 1 + 2 * part, bar_full = 2 + 2 * part;
-        const uint32_t sub_bytes = (uint32_t)(BM * p.sw * 2);
-        // 16-byte piece `piece` of output column block starting at half-relative column hc (multiple of 8) -> staging address
-        auto stage_ptr = [&](int hc) -> uint4* {
-            const int sub = hc / p.sw, cin = hc % p.sw;
-            const int piece = cin >> 3;
-            const uint32_t sw_xor = p.sw == 64 ? (uint32_t)(trow & 7) : (uint32_t)((trow >> 1) & 3);
-            return reinterpret_cast<uint4*>(my_stage + (size_t)sub * sub_bytes + (size_t)trow * (p.sw * 2) +
-                                            (((uint32_t)piece ^ sw_xor) << 4));
-        };
-        int mt, nt;
-        for (int ti = 0; gemm_tile_at(p, ti, &mt, &nt); ++ti) {
-            const int ab = ti & 1;
-            const int batch = mt / p.tiles_per_batch;
-            const int r0 = (mt % p.tiles_per_batch) * BM;
-            const int n0 = nt * p.bn;
-            const int row = r0 + lg * 32 + lane;
-            const bool valid = row < p.rows_per_batch;
-            const long long g = (long long)batch * p.rows_per_batch + row;
-            const long long off = valid ? (g / p.out_m1) * p.out_s0 + (g % p.out_m1) * p.out_s1 : 0;
-            // folded RMSNorm: 1/rms of this row of A and of the residual row, from the partial sums of squares (fixed order)
-            float r_a = 1.0f, r_res = 1.0f;
-            if (p.a_ss && valid) {
-                float ss = 0.0f;
-                for (int i = 0; i < p.a_ss_parts; ++i) ss += __ldg(p.a_ss + g * p.a_ss_parts + i);
-                r_a = rsqrtf(ss * p.norm_inv_dim + p.norm_eps);
+        return;
+    }
+
+    const int half = wg - 1;                   // rows 64 * half .. + 63 of the tile
+    const int t = threadIdx.x - 128 * wg;
+    const int lane = t & 31, quad = lane & 3;
+    const int rloc = half * 64 + (t >> 5) * 16 + (lane >> 2);   // tile rows rloc and rloc + 8
+    const int n_out_total = ACT == GEMM_ACT_SWIGLU ? p.N / 2 : p.N;
+    int s = 0;
+    uint32_t ph = 0;
+    int mt, nt;
+    for (int ti = 0; gemm_tile_at(p, ti, &mt, &nt); ++ti) {
+        float acc[BN_MAX / 32][16];
+        int prev = -1;   // stage read by the wgmma group still in flight
+        for (int kb = 0; kb < p.num_k_blocks; ++kb) {
+            tc::mbar_wait_silent(&full[s], ph);
+            const uint32_t st = tc::smem_u32(smem + s * stage_bytes);
+            const uint64_t adesc = tc::wgmma_desc_sw128(st + (uint32_t)(half * 64 * 128));
+            const uint64_t bdesc = tc::wgmma_desc_sw128(st + a_bytes);
+            tc::wgmma_fence();
+            switch (nch) {   // the chunk count as a constant: no predicated wgmma, no registers ptxas must fence
+                case 1: wgmma_k_block<1>(acc, adesc, bdesc, kb != 0); break;
+                case 2: wgmma_k_block<2>(acc, adesc, bdesc, kb != 0); break;
+                case 3: wgmma_k_block<3>(acc, adesc, bdesc, kb != 0); break;
+                default: wgmma_k_block<4>(acc, adesc, bdesc, kb != 0); break;
             }
-            if (p.res_ss && valid) {
-                float ss = 0.0f;
-                for (int i = 0; i < p.res_ss_parts; ++i) ss += __ldg(p.res_ss + g * p.res_ss_parts + i);
-                r_res = rsqrtf(ss * p.norm_inv_dim + p.norm_eps);
+            tc::wgmma_commit();
+            // one group stays in flight: the previous K block's group has completed, so its stage goes back to the producer
+            tc::wgmma_wait<1>();
+            if (prev >= 0 && t == 0) tc::mbar_arrive(&empty[prev]);
+            prev = s;
+            if (++s == STAGES) {
+                s = 0;
+                ph ^= 1;
             }
-            float ss_out = 0.0f;  // sum of squares of what this thread stores for this tile
-            if (staged && c_begin < c_end) {
-                // the stores of this set's previous tile have read its staging columns: they may be rewritten
-                if (storer) {
-                    tc::bulk_wait_group_read<0>();
-                    if (p.res_tma) {
-                        // The residual tile of this set's columns comes in by TMA, into the very staging bytes the output will
-                        // overwrite (same swizzle, so thread (row) x 16-byte piece reads and writes its own address): issued
-                        // here, it lands while the main loop of this tile still runs, and the epilogue never does the
-                        // row-per-thread global loads (32 cache lines per warp request) it would otherwise need.
-                        const int oc0 = c_begin * 32, oc1 = c_end * 32;
-                        const int nsub = (oc1 - oc0) / p.sw;
-                        tc::mbar_arrive_expect_tx(&res_full[part], (uint32_t)nsub * sub_bytes);
-                        for (int k = 0; k < nsub; ++k) {
-                            tc::tma_load_3d(my_stage + (size_t)k * sub_bytes, &tma_r, &res_full[part], n0 + oc0 + k * p.sw, r0, batch);
-                        }
-                    }
-                }
-                named_bar_sync(bar_free, 128);
-            }
-            tc::mbar_wait(&tmem_full[ab], (uint32_t)((ti >> 1) & 1));
-            tc::tc_fence_after();
-            if (p.res_tma && c_begin < c_end) tc::mbar_wait(&res_full[part], (uint32_t)(ti & 1));
-            if (c_begin == c_end) {
-                tc::tc_fence_before();
-                tc::mbar_arrive(&tmem_empty[ab]);
-            }
-            if constexpr (ACT == GEMM_ACT_ROPE) {
-                // head_dim 64 = two 32-column chunks (x1 | x2): out1 = cos*x1 - sin*x2, out2 = sin*x1 + cos*x2
-                const int tpos = (int)(g % p.rope_T);
-                const float4* tab = reinterpret_cast<const float4*>(p.rope) + tpos;  // [j][position]: (cos,sin) x 2 dims
-                for (int c = c_begin; c < c_end; c += 2) {
-                    uint32_t r0[32], r1[32];
-                    tc::tmem_ld_32x32(tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)(ab * p.bn + c * 32), r0);
-                    tc::tmem_ld_32x32(tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)(ab * p.bn + (c + 1) * 32), r1);
-                    tc::tmem_ld_wait();
-                    if (c + 2 >= c_end) {
-                        tc::tc_fence_before();
-                        tc::mbar_arrive(&tmem_empty[ab]);
-                    }
-                    const int nc = n0 + c * 32;
-                    if (valid || staged) {
-                        __half2 h0[16], h1[16];
-                        const bool rot = nc < p.rope_cols;
+        }
+        tc::wgmma_wait<0>();
+        if (t == 0) tc::mbar_arrive(&empty[prev]);
+
+        // ---- epilogue from the accumulator fragments: rows rloc (+ 8), columns 32 c + 8 j + 2 quad (+ 1)
+        const int batch = mt / p.tiles_per_batch;
+        const int r0 = (mt % p.tiles_per_batch) * BM;
+        const int n0 = nt * p.bn;
+        // 32-bit division only: a 64-bit division is a library call, and a call in this function makes ptxas serialise the
+        // wgmma pipeline.  make_gemm_plan checks that rows, strides and column blocking fit in 32 bits.
+        bool valid[2];
+        long long g[2], off[2];
+        float r_a[2], r_res[2], row_bias[2];
 #pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                            float a0 = __uint_as_float(r0[2 * j]) * r_a, a1 = __uint_as_float(r0[2 * j + 1]) * r_a;
-                            float b0 = __uint_as_float(r1[2 * j]) * r_a, b1 = __uint_as_float(r1[2 * j + 1]) * r_a;
+        for (int h = 0; h < 2; ++h) {
+            const int row = r0 + rloc + 8 * h;
+            valid[h] = row < p.rows_per_batch;
+            const uint32_t g32 = (uint32_t)(batch * p.rows_per_batch + row);
+            g[h] = g32;
+            off[h] = valid[h] ? (long long)(g32 / p.out_m1) * p.out_s0 + (long long)(g32 % p.out_m1) * p.out_s1 : 0;
+            // folded RMSNorm: 1/rms of this row of A and of the residual row, from the partial sums of squares (fixed order)
+            r_a[h] = 1.0f;
+            r_res[h] = 1.0f;
+            if (p.a_ss && valid[h]) {
+                float ss = 0.0f;
+                for (int i = 0; i < p.a_ss_parts; ++i) ss += __ldg(p.a_ss + g[h] * p.a_ss_parts + i);
+                r_a[h] = rsqrtf(ss * p.norm_inv_dim + p.norm_eps);
+            }
+            if (p.res_ss && valid[h]) {
+                float ss = 0.0f;
+                for (int i = 0; i < p.res_ss_parts; ++i) ss += __ldg(p.res_ss + g[h] * p.res_ss_parts + i);
+                r_res[h] = rsqrtf(ss * p.norm_inv_dim + p.norm_eps);
+            }
+            row_bias[h] = (p.bias && p.bias_per_row && valid[h]) ? __ldg(p.bias + g[h]) : 0.0f;
+        }
+        if constexpr (ACT == GEMM_ACT_ROPE) {
+            // head_dim 64 = two 32-column chunks (x1 | x2): out1 = cos*x1 - sin*x2, out2 = sin*x1 + cos*x2
+#pragma unroll
+            for (int c = 0; c < BN_MAX / 32; c += 2) {
+                if (c < nch) {
+                    const int nc0 = n0 + c * 32;
+                    const bool rot = nc0 < p.rope_cols;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        if (!valid[h]) continue;
+                        const float4* tab = reinterpret_cast<const float4*>(p.rope) + (int)((uint32_t)g[h] % (uint32_t)p.rope_T);
+#pragma unroll
+                        for (int j = 0; j < 4; ++j) {
+                            const int col = 8 * j + 2 * quad;   // column pair (col, col + 1) of x1; x2 is 32 columns on
+                            float a0 = acc[c][4 * j + 2 * h] * r_a[h], a1 = acc[c][4 * j + 2 * h + 1] * r_a[h];
+                            float b0 = acc[c + 1][4 * j + 2 * h] * r_a[h], b1 = acc[c + 1][4 * j + 2 * h + 1] * r_a[h];
                             if (rot) {
-                                const float4 cs = __ldg(tab + (size_t)j * p.rope_stride);
+                                const float4 cs = __ldg(tab + (size_t)(col / 2) * p.rope_stride);
                                 const float x0 = cs.x * a0 - cs.y * b0, y0 = cs.y * a0 + cs.x * b0;
                                 const float x1 = cs.z * a1 - cs.w * b1, y1 = cs.w * a1 + cs.z * b1;
                                 a0 = x0; b0 = y0; a1 = x1; b1 = y1;
                             }
-                            h0[j] = __floats2half2_rn(a0, a1);
-                            h1[j] = __floats2half2_rn(b0, b1);
-                        }
-                        if (staged) {
-                            const int hc = (c - c_begin) * 32;
-#pragma unroll
-                            for (int q = 0; q < 4; ++q) {
-                                *stage_ptr(hc + 8 * q) = *reinterpret_cast<uint4*>(&h0[4 * q]);
-                                *stage_ptr(hc + 32 + 8 * q) = *reinterpret_cast<uint4*>(&h1[4 * q]);
-                            }
-                        } else {
-                            uint4* dst = reinterpret_cast<uint4*>(p.out + off + nc);
-#pragma unroll
-                            for (int q = 0; q < 4; ++q) {
-                                dst[q] = *reinterpret_cast<uint4*>(&h0[4 * q]);
-                                dst[4 + q] = *reinterpret_cast<uint4*>(&h1[4 * q]);
-                            }
+                            *reinterpret_cast<__half2*>(p.out + off[h] + nc0 + col) = __floats2half2_rn(a0, a1);
+                            *reinterpret_cast<__half2*>(p.out + off[h] + nc0 + 32 + col) = __floats2half2_rn(b0, b1);
                         }
                     }
                 }
-            } else {
-                for (int c = c_begin; c < c_end; ++c) {
-                    uint32_t r[32];
-                    tc::tmem_ld_32x32(tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)(ab * p.bn + c * 32), r);
-                    tc::tmem_ld_wait();
-                    if (c == c_end - 1) {
-                        // accumulator fully read: hand the TMEM buffer back before the (long) math + stores
-                        tc::tc_fence_before();
-                        tc::mbar_arrive(&tmem_empty[ab]);
-                    }
-                    const int nc = n0 + c * 32;
-                    const long long coff = p.out_col_m1 > 0 ? (nc / p.out_col_m1) * p.out_col_s0 + (nc % p.out_col_m1) : nc;
-                    float v[32];
-                    const float row_bias = (p.bias && p.bias_per_row && valid) ? __ldg(p.bias + g) : 0.0f;
+            }
+        } else {
+            float ss_out[2][BN_MAX / 32];   // sums of squares of what this thread stores, per row and 32-column chunk
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) * r_a;
-                    if (p.bias) {
-                        if (p.bias_per_row) {
+            for (int c = 0; c < BN_MAX / 32; ++c) {
+                ss_out[0][c] = ss_out[1][c] = 0.0f;
+                if (c >= nch) continue;
 #pragma unroll
-                            for (int j = 0; j < 32; ++j) v[j] += row_bias;
+                for (int j = 0; j < 4; ++j) {
+                    const int nc = n0 + c * 32 + 8 * j + 2 * quad;
+                    float2 b2 = make_float2(0.0f, 0.0f);
+                    if (p.bias && !p.bias_per_row) b2 = __ldg(reinterpret_cast<const float2*>(p.bias + nc));
+                    float2 gain = make_float2(1.0f, 1.0f);
+                    if (p.residual && p.res_gain) gain = __ldg(reinterpret_cast<const float2*>(p.res_gain + nc));
+                    const long long coff = p.out_col_m1 > 0
+                            ? (long long)((uint32_t)nc / p.out_col_m1) * p.out_col_s0 + (long long)((uint32_t)nc % p.out_col_m1)
+                            : nc;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        if (!valid[h]) continue;
+                        float v0 = acc[c][4 * j + 2 * h] * r_a[h] + b2.x + row_bias[h];
+                        float v1 = acc[c][4 * j + 2 * h + 1] * r_a[h] + b2.y + row_bias[h];
+                        if constexpr (ACT == GEMM_ACT_SWIGLU) {
+                            // columns (2i, 2i + 1) = (y, gate) -> output column i
+                            p.out[off[h] + nc / 2] = __float2half_rn(v0 * swish_fast(v1));
                         } else {
-                            // the column vector is the same for every lane: 8 broadcast 16-byte loads, not 32 scalar ones
-                            const float4* bp = reinterpret_cast<const float4*>(p.bias + nc);
-#pragma unroll
-                            for (int q = 0; q < 8; ++q) {
-                                const float4 b4 = __ldg(bp + q);
-                                v[4 * q] += b4.x; v[4 * q + 1] += b4.y; v[4 * q + 2] += b4.z; v[4 * q + 3] += b4.w;
+                            if (p.residual) {
+                                const float2 f = __half22float2(
+                                        *reinterpret_cast<const __half2*>(p.residual + g[h] * (long long)n_out_total + nc));
+                                const float ar = p.alpha * r_res[h];
+                                v0 += (ar * gain.x) * f.x;
+                                v1 += (ar * gain.y) * f.y;
                             }
-                        }
-                    }
-                    if constexpr (ACT == GEMM_ACT_SWIGLU) {
-                        if (valid || staged) {
-                            __half2 h[8];
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                const float y0 = v[4 * j], g0 = v[4 * j + 1], y1 = v[4 * j + 2], g1 = v[4 * j + 3];
-                                h[j] = __floats2half2_rn(y0 * swish_fast(g0), y1 * swish_fast(g1));
-                            }
-                            if (staged) {
-                                const int hc = (c - c_begin) * 16;
-                                *stage_ptr(hc) = *reinterpret_cast<uint4*>(&h[0]);
-                                *stage_ptr(hc + 8) = *reinterpret_cast<uint4*>(&h[4]);
-                            } else {
-                                uint4* dst = reinterpret_cast<uint4*>(p.out + off + nc / 2);
-                                dst[0] = *reinterpret_cast<uint4*>(&h[0]);
-                                dst[1] = *reinterpret_cast<uint4*>(&h[4]);
-                            }
-                        }
-                    } else {
-                        if (p.residual && (valid || p.res_tma)) {
-                            const uint4* res = reinterpret_cast<const uint4*>(p.residual + g * (long long)n_out_total + nc);
-                            const float ar = p.alpha * r_res;
-                            const int hc_res = (c - c_begin) * 32;
-#pragma unroll
-                            for (int q = 0; q < 4; ++q) {
-                                const uint4 rv = p.res_tma ? *stage_ptr(hc_res + 8 * q) : __ldg(res + q);
-                                const __half2* rh = reinterpret_cast<const __half2*>(&rv);
-                                float gq[8];
-                                if (p.res_gain) {
-                                    const float4* gp4 = reinterpret_cast<const float4*>(p.res_gain + nc + q * 8);
-                                    const float4 ga = __ldg(gp4), gb = __ldg(gp4 + 1);
-                                    gq[0] = ga.x; gq[1] = ga.y; gq[2] = ga.z; gq[3] = ga.w;
-                                    gq[4] = gb.x; gq[5] = gb.y; gq[6] = gb.z; gq[7] = gb.w;
-                                } else {
-#pragma unroll
-                                    for (int j = 0; j < 8; ++j) gq[j] = 1.0f;
-                                }
-#pragma unroll
-                                for (int j = 0; j < 4; ++j) {
-                                    const float2 f = __half22float2(rh[j]);
-                                    v[q * 8 + 2 * j] += (ar * gq[2 * j]) * f.x;
-                                    v[q * 8 + 2 * j + 1] += (ar * gq[2 * j + 1]) * f.y;
-                                }
-                            }
-                        }
-                        if (valid || staged) {
-                            __half2 h[16];
-#pragma unroll
-                            for (int j = 0; j < 16; ++j) {
-                                h[j] = __floats2half2_rn(act_apply<ACT>(v[2 * j]), act_apply<ACT>(v[2 * j + 1]));
-                            }
+                            const __half2 o = __floats2half2_rn(act_apply<ACT>(v0), act_apply<ACT>(v1));
                             if (p.out_ss) {
-#pragma unroll
-                                for (int j = 0; j < 16; ++j) {
-                                    const float2 f = __half22float2(h[j]);
-                                    ss_out = fmaf(f.x, f.x, ss_out);
-                                    ss_out = fmaf(f.y, f.y, ss_out);
-                                }
+                                const float2 f = __half22float2(o);
+                                ss_out[h][c] = fmaf(f.x, f.x, ss_out[h][c]);
+                                ss_out[h][c] = fmaf(f.y, f.y, ss_out[h][c]);
                             }
-                            if (staged) {
-                                const int hc = (c - c_begin) * 32;
-#pragma unroll
-                                for (int q = 0; q < 4; ++q) *stage_ptr(hc + 8 * q) = *reinterpret_cast<uint4*>(&h[4 * q]);
-                            } else {
-                                uint4* dst = reinterpret_cast<uint4*>(p.out + off + coff);
-#pragma unroll
-                                for (int q = 0; q < 4; ++q) dst[q] = *reinterpret_cast<uint4*>(&h[4 * q]);
-                            }
+                            *reinterpret_cast<__half2*>(p.out + off[h] + coff) = o;
                         }
                     }
                 }
             }
-            if (p.out_ss && valid && c_begin < c_end) {
-                // one partial per (column tile, part): consumers add them in index order
-                p.out_ss[g * (long long)(p.n_tiles * GEMM_PARTS) + nt * GEMM_PARTS + part] = ss_out;
-            }
-            if (staged && c_begin < c_end) {
-                tc::fence_proxy_async_smem();   // staged tile -> visible to the TMA store
-                named_bar_sync(bar_full, 128);
-                if (storer) {
-                    // this set's output columns [oc0, oc1) of the tile, as sub-tiles of p.sw columns
-                    const int oc0 = c_begin * 32 / out_div, oc1 = c_end * 32 / out_div;
-                    const int col0 = n0 / out_div + oc0;
-                    const int nsub = (oc1 - oc0) / p.sw;
-                    for (int k = 0; k < nsub; ++k) {
-                        const uint8_t* src = my_stage + (size_t)k * sub_bytes;
-                        const int col = col0 + k * p.sw;
-                        if (p.out_kind == 0) {
-                            tc::tma_store_3d(&tma_o, src, col, r0, batch);
-                        } else if (p.out_kind == 1) {
-                            tc::tma_store_3d(&tma_o, src, col, r0 % p.out_P, r0 / p.out_P);
-                        } else {
-                            tc::tma_store_3d(&tma_o, src, 0, r0, col / 32);
-                        }
+            if (p.out_ss) {
+                // one partial per (column tile, 32-column chunk): the four lanes of a quad hold a row's columns
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                    for (int c = 0; c < GEMM_PARTS; ++c) {
+                        float v = ss_out[h][c];
+                        v += __shfl_xor_sync(0xffffffffu, v, 1);
+                        v += __shfl_xor_sync(0xffffffffu, v, 2);
+                        if (quad == 0 && valid[h]) p.out_ss[g[h] * (long long)(p.n_tiles * GEMM_PARTS) + nt * GEMM_PARTS + c] = v;
                     }
-                    tc::bulk_commit_group();
                 }
             }
         }
-        if (storer) tc::bulk_wait_group<0>();
     }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tc::tmem_dealloc(tmem_base, p.tmem_cols);
 }
 
 using EncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -555,85 +352,9 @@ CUtensorMap make_tmap_3d(const void* base, uint64_t d0, uint64_t d1, uint64_t d2
     return encode(base, 3, dims, strides, box, swz);
 }
 
-// Decide whether the epilogue can leave through shared memory + TMA stores: the output must be expressible as a 3-D tensor
-// (columns, rows, outer) whose 128-row tiles never straddle the outer dimension, and each epilogue warp set's column range
-// must split into sub-tiles of 64 (128-byte swizzle) or 32 (64-byte swizzle) columns.
-static void plan_output_staging(GemmPlan& p) {
-    const GemmDesc& d = p.d;
-    p.staged = 0;
-    static const bool direct = [] {
-        const char* e = std::getenv("B200_GEMM_DIRECT");  // A/B switch: per-thread global stores
-        return e && std::atoi(e) != 0;
-    }();
-    if (direct) return;
-    // measured on B200 (profiles/r02_b7_*): the staged epilogue wins wherever the epilogue bounds the tile (K = 512 with plain,
-    // bias, residual or rotary epilogues: 1.2-2.2x), and loses a little where the ring depth matters more than the stores
-    // (SwiGLU halves the output; K >= 1024 hides the epilogue under the main loop): those keep the per-thread stores and 4 stages
-    static const bool stage_all = [] {
-        const char* e = std::getenv("B200_GEMM_STAGE_ALL");  // A/B switch: stage K >= 1024 GEMMs too (3-stage ring)
-        return e && std::atoi(e) != 0;
-    }();
-    if (d.act == GEMM_ACT_SWIGLU || (d.K >= 1024 && !stage_all)) return;
-    const int nch = p.bn / 32;
-    const int out_div = d.act == GEMM_ACT_SWIGLU ? 2 : 1;
-    // every part's output width must split into sub-tiles of sw columns
-    int sw = 64;
-    for (int part = 0; part < GEMM_PARTS; ++part) {
-        int cb = 0, ce = 0;
-        gemm_part_range(nch, d.act == GEMM_ACT_ROPE ? 2 : 1, part, &cb, &ce);
-        const int w = (ce - cb) * 32 / out_div, o = cb * 32 / out_div;
-        if (w == 0) continue;
-        while (sw >= 32 && (w % sw != 0 || o % sw != 0)) sw /= 2;
-    }
-    if (sw < 32) return;
-    const uint64_t ncols = (uint64_t)(d.N / out_div);
-    uint64_t dims[3], strides[2];
-    uint32_t box[3] = {(uint32_t)sw, (uint32_t)BM, 1};
-    if (d.out_col_m1 > 0) {
-        if (d.out_col_m1 != 32 || d.out_m1 != 1 || d.batches != 1 || out_div != 1) return;
-        sw = 32;
-        box[0] = 32;
-        dims[0] = 32; dims[1] = (uint64_t)d.rows_per_batch; dims[2] = ncols / 32;
-        strides[0] = (uint64_t)d.out_s0 * 2; strides[1] = (uint64_t)d.out_col_s0 * 2;
-        p.out_kind = 2;
-    } else if (d.batches > 1) {
-        if (d.out_m1 != d.rows_per_batch) return;
-        dims[0] = ncols; dims[1] = (uint64_t)d.rows_per_batch; dims[2] = (uint64_t)d.batches;
-        strides[0] = (uint64_t)d.out_s1 * 2; strides[1] = (uint64_t)d.out_s0 * 2;
-        p.out_kind = 0;
-    } else if (d.out_m1 == 1) {
-        dims[0] = ncols; dims[1] = (uint64_t)d.rows_per_batch; dims[2] = 1;
-        strides[0] = (uint64_t)d.out_s0 * 2; strides[1] = (uint64_t)d.out_s0 * 2 * (uint64_t)d.rows_per_batch;
-        p.out_kind = 0;
-    } else if (d.out_m1 % BM == 0 && d.rows_per_batch % d.out_m1 == 0) {
-        dims[0] = ncols; dims[1] = (uint64_t)d.out_m1; dims[2] = (uint64_t)(d.rows_per_batch / d.out_m1);
-        strides[0] = (uint64_t)d.out_s1 * 2; strides[1] = (uint64_t)d.out_s0 * 2;
-        p.out_kind = 1;
-        p.out_P = (int)d.out_m1;
-    } else {
-        return;
-    }
-    if (strides[0] % 16 != 0 || strides[1] % 16 != 0 || (reinterpret_cast<uintptr_t>(d.out) & 15) != 0) return;
-    if (dims[2] > 1 && strides[1] == 0) return;
-    p.tma_o = encode(d.out, 3, dims, strides, box, sw == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B);
-    p.sw = sw;
-    p.staged = 1;
-    // the residual is dense [batches * rows][N]; per batch so that a tile's rows beyond the batch are clipped (zero-filled)
-    static const bool res_ldg = [] {
-        const char* e = std::getenv("B200_GEMM_RES_LDG");  // A/B switch: residual by per-thread global loads
-        return e && std::atoi(e) != 0;
-    }();
-    if (d.residual && out_div == 1 && !res_ldg && (reinterpret_cast<uintptr_t>(d.residual) & 15) == 0 && (ncols * 2) % 16 == 0) {
-        const uint64_t rdims[3] = {ncols, (uint64_t)d.rows_per_batch, (uint64_t)d.batches};
-        const uint64_t rstrides[2] = {ncols * 2, ncols * 2 * (uint64_t)d.rows_per_batch};
-        p.tma_r = encode(d.residual, 3, rdims, rstrides, box, sw == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B);
-        p.res_tma = 1;
-    }
-}
-
 static int pick_bn(int N) {
-    // largest tile width <= 256 that divides N and is a multiple of 32
-    for (int bn = 256; bn >= 32; bn -= 32) {
+    // largest tile width <= BN_MAX that divides N and is a multiple of 32
+    for (int bn = BN_MAX; bn >= 32; bn -= 32) {
         if (N % bn == 0) return bn;
     }
     return 0;
@@ -655,59 +376,30 @@ GemmPlan make_gemm_plan(const GemmDesc& d) {
     GemmPlan p{};
     p.d = d;
     p.bn = pick_bn(d.N);
-    if (d.N / p.bn < 2 && d.N >= 128 && (long long)d.batches * ((d.rows_per_batch + BM - 1) / BM) < 96) {
+    if (d.N / p.bn < 2 && d.N >= 128 && (long long)d.batches * ((d.rows_per_batch + BM - 1) / BM) < kNumSMs / 2) {
         p.bn = pick_bn(d.N / 2);  // few row tiles: split N further to fill more SMs
     }
     if (p.bn == 0) throw std::invalid_argument("gemm: no valid tile width");
     if (d.out_ss) {
-        // every part of every column tile must own columns, so that each partial slot is written
-        if (p.bn != pick_bn(d.N) || p.bn / 32 < GEMM_PARTS || d.act == GEMM_ACT_SWIGLU || d.act == GEMM_ACT_ROPE) {
-            throw std::invalid_argument("gemm: out_ss needs a plain epilogue and tiles of at least 128 columns");
+        // every 32-column chunk of every column tile owns one partial slot
+        if (p.bn != pick_bn(d.N) || p.bn / 32 != GEMM_PARTS || d.act == GEMM_ACT_SWIGLU || d.act == GEMM_ACT_ROPE) {
+            throw std::invalid_argument("gemm: out_ss needs a plain epilogue and tiles of 128 columns");
         }
     }
     if ((d.a_ss && (d.a_ss_parts < 1 || d.norm_dim < 1)) || (d.res_ss && (d.res_ss_parts < 1 || d.norm_dim < 1 || !d.residual))) {
         throw std::invalid_argument("gemm: folded RMSNorm needs the partial count, the norm dimension and a residual");
     }
     if (d.act == GEMM_ACT_SWIGLU && (p.bn % 64) != 0) throw std::invalid_argument("gemm: swiglu needs BN % 64 == 0");
-    if (d.act == GEMM_ACT_ROPE && ((p.bn % 128) != 0 || !d.rope || d.rope_T <= 0)) {
-        throw std::invalid_argument("gemm: rope epilogue needs BN % 128 == 0 and a table");
+    if (d.act == GEMM_ACT_ROPE && ((p.bn % 64) != 0 || !d.rope || d.rope_T <= 0)) {
+        throw std::invalid_argument("gemm: rope epilogue needs BN % 64 == 0 and a table");
     }
     p.tiles_per_batch = (d.rows_per_batch + BM - 1) / BM;
-    // Operand-stationary schedules (1: W resident, 2: A resident): 128-column tiles, the CTA's slice of the small operand
-    // (K / 64 blocks of 16 KB) resident in front of a ring that then carries the other operand alone.  Built on the theory
-    // that the K <= 512 GEMMs are bound by L2 -> SM operand traffic; measured and REJECTED (battery 22, parity green): the
-    // hac x-projection 1.75 -> 1.99 ms, sup QKV+RoPE 0.27 -> 0.48 ms, FC1+SwiGLU 0.46 -> 0.61 ms.  The 128-column tile halves
-    // the work per epilogue hand-over (and leaves two of the four epilogue warp sets idle in the rotary epilogue), and that,
-    // not operand traffic, is what these GEMMs are short of; the x-projection's real problem was its tile order (above).
-    // The schedule stays in the kernel as an experiment switch: B200_GEMM_WSTAT=1 (W resident) or 2 (A resident) applies it to
-    // every GEMM whose shape qualifies.
-    static const int wstat_mode = [] {
-        const char* e = std::getenv("B200_GEMM_WSTAT");
-        const int v = e ? std::atoi(e) : 0;
-        return v == 1 || v == 2 ? v : 0;
-    }();
-    const long long m_tiles = (long long)p.tiles_per_batch * d.batches;
-    if (wstat_mode && !d.out_ss && d.N % 128 == 0 && d.K / BK <= 8) {
-        const long long fixed = wstat_mode == 1 ? d.N / 128 : m_tiles;      // tiles along the resident operand
-        const long long walked = wstat_mode == 1 ? m_tiles : d.N / 128;
-        if (fixed <= kNumSMs / 2 && walked >= 4 * (kNumSMs / fixed)) {
-            p.bn = 128;
-            p.wstat = wstat_mode;
-        }
+    if ((long long)p.tiles_per_batch * BM * d.batches >= (1LL << 31) || d.out_m1 < 1 || d.out_m1 >= (1LL << 32) ||
+        d.out_col_m1 < 0 || d.out_col_m1 >= (1LL << 32)) {
+        throw std::invalid_argument("gemm: rows and output blocking must fit 32-bit index arithmetic");
     }
     p.grid = dim3((unsigned)(p.tiles_per_batch * d.batches), (unsigned)(d.N / p.bn), 1);
-    plan_output_staging(p);
-    const size_t w_res_bytes = p.wstat ? (size_t)(d.K / BK) * (p.wstat == 1 ? p.bn : BM) * BK * 2 : 0;
-    const size_t stage_bytes = (p.wstat == 2 ? 0 : (size_t)BM * BK * 2) + (p.wstat == 1 ? 0 : (size_t)p.bn * BK * 2);
-    const size_t staging = p.staged ? (size_t)BM * (p.bn / (d.act == GEMM_ACT_SWIGLU ? 2 : 1)) * 2 : 0;
-    p.stages = STAGES;
-    if (w_res_bytes + (size_t)p.stages * stage_bytes + staging + 256 + 1024 > 227 * 1024) p.stages = 3;
-    p.smem = w_res_bytes + (size_t)p.stages * stage_bytes + staging + 256 + 1024;
-    if (p.smem > 227 * 1024) {
-        p.staged = 0;
-        p.stages = STAGES;
-        p.smem = w_res_bytes + (size_t)p.stages * stage_bytes + 256 + 1024;
-    }
+    p.smem = (size_t)STAGES * ((size_t)BM * BK * 2 + (size_t)p.bn * BK * 2) + 256 + 1024;
     if (p.smem > 227 * 1024) throw std::logic_error("gemm: shared-memory plan does not fit");
     const uint64_t batch_stride = d.batches > 1 ? (uint64_t)d.a_batch_stride * 2 : (uint64_t)d.a_row_stride * 2 * d.rows_per_batch;
     p.tma_a = make_tmap_3d(d.a, (uint64_t)(d.a_inner > 0 ? d.a_inner : d.K), (uint64_t)d.rows_per_batch, (uint64_t)d.batches, (uint64_t)d.a_row_stride * 2,
@@ -717,10 +409,10 @@ GemmPlan make_gemm_plan(const GemmDesc& d) {
 }
 
 template <int ACT>
-static void launch_gemm(int grid, size_t smem, cudaStream_t stream, const CUtensorMap& a, const CUtensorMap& w, const CUtensorMap& o,
-                        const CUtensorMap& r, const GemmKernelParams& k) {
-    ensure_dynamic_smem(gemm_f16_tcgen05_kernel<ACT>, 227 * 1024);
-    gemm_f16_tcgen05_kernel<ACT><<<grid, GEMM_THREADS, smem, stream>>>(a, w, o, r, k);
+static void launch_gemm(int grid, size_t smem, cudaStream_t stream, const CUtensorMap& a, const CUtensorMap& w,
+                        const GemmKernelParams& k) {
+    ensure_dynamic_smem(gemm_f16_wgmma_kernel<ACT>, 227 * 1024);
+    gemm_f16_wgmma_kernel<ACT><<<grid, GEMM_THREADS, smem, stream>>>(a, w, k);
 }
 
 void run_gemm(const GemmPlan& p, cudaStream_t stream) {
@@ -730,13 +422,12 @@ void run_gemm(const GemmPlan& p, cudaStream_t stream) {
     k.N = p.d.N;
     k.num_k_blocks = p.d.K / BK;
     k.bn = p.bn;
-    k.act = p.d.act;
     k.bias = p.d.bias;
     k.out = p.d.out;
-    k.out_m1 = p.d.out_m1;
+    k.out_m1 = (uint32_t)p.d.out_m1;
     k.out_s0 = p.d.out_s0;
     k.out_s1 = p.d.out_s1;
-    k.out_col_m1 = p.d.out_col_m1;
+    k.out_col_m1 = (uint32_t)p.d.out_col_m1;
     k.out_col_s0 = p.d.out_col_s0;
     k.bias_per_row = p.d.bias_per_row;
     k.rope = p.d.rope;
@@ -745,11 +436,10 @@ void run_gemm(const GemmPlan& p, cudaStream_t stream) {
     k.rope_stride = p.d.rope_stride;
     k.residual = p.d.residual;
     k.alpha = p.d.alpha;
-    uint32_t cols = 32;
-    while ((int)cols < 2 * p.bn) cols <<= 1;  // double-buffered accumulator
-    k.tmem_cols = cols;
     k.n_tiles = p.d.N / p.bn;
-    k.num_tiles = p.tiles_per_batch * p.d.batches * k.n_tiles;
+    k.m_tiles = p.tiles_per_batch * p.d.batches;
+    k.num_tiles = k.m_tiles * k.n_tiles;
+    k.mfast = k.m_tiles < k.n_tiles ? 1 : 0;
     k.out_ss = p.d.out_ss;
     k.a_ss = p.d.a_ss;
     k.res_ss = p.d.res_ss;
@@ -758,42 +448,16 @@ void run_gemm(const GemmPlan& p, cudaStream_t stream) {
     k.res_ss_parts = p.d.res_ss_parts;
     k.norm_inv_dim = p.d.norm_dim > 0 ? 1.0f / (float)p.d.norm_dim : 0.0f;
     k.norm_eps = p.d.norm_eps;
-    k.staged = p.staged;
-    k.stages = p.stages;
-    k.sw = p.sw;
-    k.out_kind = p.out_kind;
-    k.out_P = p.out_P > 0 ? p.out_P : 1;
-    static const int env_ctas = [] {
-        const char* e = std::getenv("B200_GEMM_MAX_CTAS");  // experiments: overrides every plan's cap
-        const int v = e ? std::atoi(e) : 0;
-        return v > 0 && v < kNumSMs ? v : 0;
-    }();
-    int max_ctas = env_ctas > 0 ? env_ctas : (p.d.max_ctas > 0 && p.d.max_ctas < kNumSMs ? p.d.max_ctas : kNumSMs);
-    int grid = k.num_tiles < max_ctas ? k.num_tiles : max_ctas;
-    k.wstat = p.wstat;
-    k.m_tiles = p.tiles_per_batch * p.d.batches;
-    static const bool no_mfast = [] {
-        const char* e = std::getenv("B200_GEMM_NFAST");  // A/B switch: column tile always fastest (the old order)
-        return e && std::atoi(e) != 0;
-    }();
-    k.mfast = (k.m_tiles < k.n_tiles && !no_mfast) ? 1 : 0;
-    if (p.wstat) {
-        // every CTA owns one tile of the resident operand: the grid is a multiple of the number of those tiles
-        const int fixed = p.wstat == 1 ? k.n_tiles : k.m_tiles;
-        grid = (max_ctas / fixed) * fixed;
-        if (grid < fixed) grid = fixed;
-    }
-    const CUtensorMap& tmo = p.staged ? p.tma_o : p.tma_a;
-    const CUtensorMap& tmr = p.staged && p.res_tma ? p.tma_r : p.tma_a;
-    k.res_tma = p.staged && p.res_tma;
+    const int max_ctas = p.d.max_ctas > 0 && p.d.max_ctas < kNumSMs ? p.d.max_ctas : kNumSMs;
+    const int grid = k.num_tiles < max_ctas ? k.num_tiles : max_ctas;
     switch (p.d.act) {
-        case GEMM_ACT_NONE: launch_gemm<GEMM_ACT_NONE>(grid, p.smem, stream, p.tma_a, p.tma_w, tmo, tmr, k); break;
-        case GEMM_ACT_SWISH: launch_gemm<GEMM_ACT_SWISH>(grid, p.smem, stream, p.tma_a, p.tma_w, tmo, tmr, k); break;
-        case GEMM_ACT_SWISH_CLAMP: launch_gemm<GEMM_ACT_SWISH_CLAMP>(grid, p.smem, stream, p.tma_a, p.tma_w, tmo, tmr, k); break;
-        case GEMM_ACT_TANH: launch_gemm<GEMM_ACT_TANH>(grid, p.smem, stream, p.tma_a, p.tma_w, tmo, tmr, k); break;
-        case GEMM_ACT_TANH_X5: launch_gemm<GEMM_ACT_TANH_X5>(grid, p.smem, stream, p.tma_a, p.tma_w, tmo, tmr, k); break;
-        case GEMM_ACT_SWIGLU: launch_gemm<GEMM_ACT_SWIGLU>(grid, p.smem, stream, p.tma_a, p.tma_w, tmo, tmr, k); break;
-        case GEMM_ACT_ROPE: launch_gemm<GEMM_ACT_ROPE>(grid, p.smem, stream, p.tma_a, p.tma_w, tmo, tmr, k); break;
+        case GEMM_ACT_NONE: launch_gemm<GEMM_ACT_NONE>(grid, p.smem, stream, p.tma_a, p.tma_w, k); break;
+        case GEMM_ACT_SWISH: launch_gemm<GEMM_ACT_SWISH>(grid, p.smem, stream, p.tma_a, p.tma_w, k); break;
+        case GEMM_ACT_SWISH_CLAMP: launch_gemm<GEMM_ACT_SWISH_CLAMP>(grid, p.smem, stream, p.tma_a, p.tma_w, k); break;
+        case GEMM_ACT_TANH: launch_gemm<GEMM_ACT_TANH>(grid, p.smem, stream, p.tma_a, p.tma_w, k); break;
+        case GEMM_ACT_TANH_X5: launch_gemm<GEMM_ACT_TANH_X5>(grid, p.smem, stream, p.tma_a, p.tma_w, k); break;
+        case GEMM_ACT_SWIGLU: launch_gemm<GEMM_ACT_SWIGLU>(grid, p.smem, stream, p.tma_a, p.tma_w, k); break;
+        case GEMM_ACT_ROPE: launch_gemm<GEMM_ACT_ROPE>(grid, p.smem, stream, p.tma_a, p.tma_w, k); break;
         default: throw std::invalid_argument("gemm: unknown activation");
     }
     B200_CUDA(cudaGetLastError());
@@ -804,7 +468,7 @@ void run_gemm(const GemmPlan& p, cudaStream_t stream) {
 // ------------------------------------------------------------------------------------------------
 void test_gemm_host(int device, const uint16_t* a, const uint16_t* b, const float* bias, int M, int N, int K, int activation,
                     uint16_t* c) {
-    require_sm100(device);
+    require_sm90(device);
     const int Kp = (K + BK - 1) / BK * BK;
     const int n_out = activation == GEMM_ACT_SWIGLU ? N / 2 : N;
     Arena arena;

@@ -1,5 +1,5 @@
-// tcgen05 GEMM with fused epilogue:  out[row(g)][n] = act( sum_k A[g][k] * W[n][k] + bias[n] ), fp16 in/out,
-// fp32 accumulation in TMEM.  See gemm.cu.
+// wgmma GEMM with fused epilogue:  out[row(g)][n] = act( sum_k A[g][k] * W[n][k] + bias[n] ), fp16 in/out,
+// fp32 accumulation in registers.  See gemm.cu.
 #pragma once
 
 #include "tc.cuh"
@@ -68,15 +68,11 @@ struct GemmDesc {
 
 struct GemmPlan {
     CUtensorMap tma_a, tma_w;
-    CUtensorMap tma_o;   // output, when the epilogue leaves through shared memory + TMA stores (staged)
-    CUtensorMap tma_r;   // residual [batches][rows][N], TMA-loaded into the staging tile ahead of the epilogue (res_tma)
     GemmDesc d;
     int bn = 128;
     int tiles_per_batch = 0;
     dim3 grid;
     size_t smem = 0;
-    int staged = 0, stages = 4, sw = 64, out_kind = 0, out_P = 1, res_tma = 0;
-    int wstat = 0;   // operand-stationary schedule in effect (experiment switch B200_GEMM_WSTAT, gemm.cu): 1 = W resident, 2 = A
 };
 
 GemmPlan make_gemm_plan(const GemmDesc& d);

@@ -1,11 +1,10 @@
-// Conv -> LSTM -> linear CRF forward (fast / hac models) for sm_100a.
+// Conv -> LSTM -> linear CRF forward (fast / hac models) for sm_90a.
 //
 // Replaces, for the CUDA path of dorado/basecall/model/CRFModel.cpp:69-115:
 //   ConvStack layers 1,2   host_convolution_f16              dorado/nn/ConvStack.cpp:216-232  -> conv12_tc_kernel (conv2 on
-//                                                                                         tcgen05; v5 shapes), conv12_kernel (FMA pipe)
+//                                                                                         mma.sync; v5 shapes), conv12_kernel (FMA pipe)
 //   ConvStack layer 3      host_linear "cutlass conv"        dorado/nn/ConvStack.cpp:236-275  -> gemm.cu
-//   LSTMStack              host_cutlass_lstm/host_small_lstm dorado/nn/LSTMStack.cpp:127-238 -> lstm_layer_kernel (C = 96),
-//                                                                                         gx GEMM + lstm_cluster_kernel (C = 192, 384)
+//   LSTMStack              host_cutlass_lstm/host_small_lstm dorado/nn/LSTMStack.cpp:127-238 -> gx GEMM + lstm_rec_kernel
 //   LinearCRF              host_linear                       dorado/nn/CRFModules.cpp:49-122   -> gemm.cu
 // Semantics are those of the CPU modules (ConvStack.cpp:146-163, LSTMStack.cpp:29-41, CRFModules.cpp:24-34).
 //
@@ -24,6 +23,10 @@
 #include <cstdlib>
 #include <cstring>
 #include <vector>
+
+#include <cooperative_groups.h>
+
+namespace cg = cooperative_groups;
 
 namespace b200 {
 
@@ -134,44 +137,38 @@ __global__ void __launch_bounds__(CONV_TT) conv12_kernel(const Conv12Params p) {
 // conv1 + conv2 with conv2 on the tensor cores (the v5 shape: conv1 1 -> 16, conv2 16 -> 16 with 5 taps).
 //
 // conv2 is 1280 of the 1360 multiply-adds per sample; on the FMA pipe (conv12_kernel above) that is 1.4e10 FLOP per batch of
-// 512 x 9996 samples and the kernel sat at 4 % of the HBM roofline it should be bound by (2 B in, 32 B out per sample).  Here a
-// tile of 128 output samples is one M = 128, N = 16, K = 80 contraction on tcgen05:
+// 512 x 9996 samples for a kernel that should be bound by HBM (2 B in, 32 B out per sample).  Here a tile of 128 output
+// samples is one M = 128, N = 16, K = 80 contraction on mma.sync:
 //   * conv1 (+ activation) runs on the FMA pipe, one thread per conv1 position, and its 16 channels are rounded to fp16
 //     (every activation tensor between layers is fp16, as in the reference's CUDA path);
-//   * the A operand is conv2's im2col tile built directly in shared memory in the 128-byte-swizzled K-major layout:
+//   * the A operand is conv2's im2col tile built directly in shared memory in a 128-byte-swizzled K-major layout:
 //     K index = tap * 16 + channel, so the 32 bytes of conv1 position j go to row j - tap, 16-byte chunks 2 tap and 2 tap + 1
-//     (five 2 x 16 B stores per thread; the XOR swizzle keeps the eight rows of a phase on distinct banks);
-//   * B = the conv2 weights [16][80] fp16 in the same layout, written once per CTA; the accumulator is 16 TMEM columns;
-//   * four warps read the accumulator back (thread = output sample), add the bias, apply the activation and store the
-//     sample's 16 fp16 channels as one 32-byte row: a warp writes 1 KB contiguous.
-// The phases of a tile are separated by CTA barriers; five CTAs fit an SM (37 KB shared memory, 32 TMEM columns, 12288
-// registers each) and hide each other's barrier and MMA latency.  The grid is persistent and takes tiles from a counter.
+//     (five 2 x 16 B stores per thread; the XOR swizzle keeps the eight rows of an ldmatrix phase on distinct banks);
+//   * B = the conv2 weights [16][80] fp16 in the same layout, written once per CTA and held in registers as mma fragments;
+//   * warps 0-3 each contract 32 rows (2 x 2 m16n8k16 tiles, 5 K steps), add the bias, apply the activation and store
+//     the samples' 16 fp16 channels.
+// The phases of a tile are separated by CTA barriers; several CTAs share an SM and hide each other's barriers.  The grid
+// is persistent and takes tiles from a counter.
 // ------------------------------------------------------------------------------------------------
 constexpr int C12_TILE = 128;
-// warps 0-3: conv1 producers and epilogue (TMEM lane quarter = warp); warp 4: tail positions + MMA issue; warp 5 only pads the
-// CTA to 192 threads x 64 registers = 12288 registers: more than the recurrence kernels leave free on their SMs (fast: 8192,
-// hac: 10240).  Those kernels hold all 512 tensor-memory columns for a whole layer, and a CTA of this kernel placed beside one
-// would sit in tcgen05.alloc until that layer ends.  Tiles are also handed out dynamically (atomic counter), so a CTA that
-// does get stuck holds no work.
+// warps 0-3: conv1 producers, MMA and epilogue (32 rows each); warp 4: conv1 tail positions; warp 5 idle
 constexpr int C12_THREADS = 192;
 constexpr int C12_SMEM = 2 * 16384 + 2 * 2048 + 1024;  // A (2 k-blocks of 128 rows x 128 B), B (2 k-blocks of 16 rows), alignment slack
 
-__global__ void __launch_bounds__(C12_THREADS, 5) conv12_tc_kernel(const Conv12Params p, int tiles_per_chunk, int num_tiles) {
+__global__ void __launch_bounds__(C12_THREADS, 4) conv12_tc_kernel(const Conv12Params p, int tiles_per_chunk, int num_tiles) {
     extern __shared__ __align__(1024) uint8_t c12_smem_raw[];
     uint8_t* smem = c12_smem_raw + ((1024u - (tc::smem_u32(c12_smem_raw) & 1023u)) & 1023u);
     uint8_t* a_tile = smem;               // [2][128 rows][128 B]
     uint8_t* b_tile = smem + 2 * 16384;   // [2][16 rows][128 B]
     __shared__ float xs[C12_TILE + 4 + 2 * MAXW];
     __shared__ float s_w1[16 * MAXW], s_b1[16], s_b2[16];
-    __shared__ uint64_t mma_done;
-    __shared__ uint32_t tmem_holder;
     __shared__ int s_tile;
     const ConvAct a1 = conv_act_coef(p.act1), a2 = conv_act_coef(p.act2);
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int p1 = p.w1 / 2;
     constexpr int p2 = 2;
 
-    // ---- once per CTA: conv1 weights / biases, conv2 weights as the fp16 B operand, barrier, tensor memory
+    // ---- once per CTA: conv1 weights / biases, conv2 weights as the fp16 B operand
     for (int i = tid; i < 16 * MAXW; i += C12_THREADS) s_w1[i] = __ldg(p.w + i);
     if (tid < 16) {
         s_b1[tid] = __ldg(p.w + 16 * MAXW + tid);
@@ -188,23 +185,20 @@ __global__ void __launch_bounds__(C12_THREADS, 5) conv12_tc_kernel(const Conv12P
                     __float2half_rn(__ldg(w2 + (tap * 16 + ci) * 16 + co));
         }
     }
-    if (tid == 0) {
-        tc::mbar_init(&mma_done, 1);
-        tc::fence_barrier_init();
-    }
-    if (warp == 4) tc::tmem_alloc(&tmem_holder, 32);
-    tc::fence_proxy_async_smem();
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_acc = tmem_holder;
-    const uint64_t adesc0 = tc::umma_desc_sw128(tc::smem_u32(a_tile));
-    const uint64_t bdesc0 = tc::umma_desc_sw128(tc::smem_u32(b_tile));
-    constexpr uint32_t idesc = tc::umma_idesc_f16(128, 16);
+    // B fragments of the five K steps: matrix q of ldmatrix.x4 = (n tile q / 2, k half q % 2)
+    uint32_t bfrag[5][4];
+    if (warp < 4) {
+        const int q = lane >> 3, r = lane & 7;
+#pragma unroll
+        for (int tap = 0; tap < 5; ++tap) {
+            const int chunk = 2 * tap + (q & 1);
+            tc::ldmatrix_x4(bfrag[tap], tc::smem_u32(b_tile + (chunk >> 3) * 2048 + tc::sw128_offset((q >> 1) * 8 + r, chunk & 7)));
+        }
+    }
 
-    uint32_t parity = 0;
     for (;;) {
-        __syncthreads();  // the previous tile's accumulator has been read and its MMAs have read A: both may be overwritten
+        __syncthreads();  // the previous tile's MMAs have read A: it may be overwritten
         if (tid == 0) s_tile = atomicAdd(p.tile_counter, 1);
         __syncthreads();
         const int tile = s_tile;
@@ -251,104 +245,54 @@ __global__ void __launch_bounds__(C12_THREADS, 5) conv12_tc_kernel(const Conv12P
                 }
             }
         }
-        tc::fence_proxy_async_smem();
         __syncthreads();
-        // ---- conv2: five K = 16 steps (one per tap), issued by one thread
-        if (tid == 128) {
-            tc::tc_fence_after();
+        // ---- conv2: warp w contracts rows 32 w .. 32 w + 31, thread = fragment rows lane / 4 (+ 8), channels 2 (lane % 4) (+ 1, + 8)
+        if (warp < 4) {
+            float acc[2][2][4];
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+                for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) acc[mt][nt][e] = 0.0f;
+            const int q = lane >> 3, r = lane & 7;
 #pragma unroll
             for (int tap = 0; tap < 5; ++tap) {
-                const uint64_t off = (uint64_t)(((tap >> 2) * 16384) >> 4) + (uint64_t)(2 * (tap & 3));
-                const uint64_t boff = (uint64_t)(((tap >> 2) * 2048) >> 4) + (uint64_t)(2 * (tap & 3));
-                tc::umma_f16(tmem_acc, adesc0 + off, bdesc0 + boff, idesc, tap != 0);
-            }
-            tc::umma_commit(&mma_done);
-        }
-        // ---- epilogue: thread = output sample
-        if (warp < 4) {
-            tc::mbar_wait(&mma_done, parity);
-            tc::tc_fence_after();
-            uint32_t r[16];
-            tc::tmem_ld_32x16(tmem_acc + ((uint32_t)(warp * 32) << 16), r);
-            tc::tmem_ld_wait();
-            const int t = t0 + tid;
-            if (t < p.T) {
-                __half2 o[8];
 #pragma unroll
-                for (int c2 = 0; c2 < 8; ++c2) {
-                    o[c2] = __floats2half2_rn(conv_act(__uint_as_float(r[2 * c2]) + s_b2[2 * c2], a2),
-                                              conv_act(__uint_as_float(r[2 * c2 + 1]) + s_b2[2 * c2 + 1], a2));
+                for (int mt = 0; mt < 2; ++mt) {
+                    // matrix q of ldmatrix.x4 = (row half q % 2, k half q / 2): the a0..a3 order of m16n8k16
+                    const int row = warp * 32 + mt * 16 + (q & 1) * 8 + r, chunk = 2 * tap + (q >> 1);
+                    uint32_t a[4];
+                    tc::ldmatrix_x4(a, tc::smem_u32(a_tile + (chunk >> 3) * 16384 + tc::sw128_offset(row, chunk & 7)));
+                    tc::mma_f16_16816(acc[mt][0], a, bfrag[tap][0], bfrag[tap][1]);
+                    tc::mma_f16_16816(acc[mt][1], a, bfrag[tap][2], bfrag[tap][3]);
                 }
-                if (t >= L) {  // beyond a short chunk's end: the next convolution's zero padding
-#pragma unroll
-                    for (int c2 = 0; c2 < 8; ++c2) o[c2] = __floats2half2_rn(0.0f, 0.0f);
-                }
-                uint4* dst = reinterpret_cast<uint4*>(p.out + ((size_t)n * p.T_pad + p.front_pad + t) * 16);
-                dst[0] = *reinterpret_cast<uint4*>(&o[0]);
-                dst[1] = *reinterpret_cast<uint4*>(&o[4]);
             }
-            tc::tc_fence_before();
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt) {
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                    const int t = t0 + warp * 32 + mt * 16 + (lane >> 2) + 8 * hh;
+                    if (t >= p.T) continue;
+                    __half* dst = p.out + ((size_t)n * p.T_pad + p.front_pad + t) * 16;
+#pragma unroll
+                    for (int nt = 0; nt < 2; ++nt) {
+                        const int co = nt * 8 + 2 * (lane & 3);
+                        __half2 o = __floats2half2_rn(conv_act(acc[mt][nt][2 * hh] + s_b2[co], a2),
+                                                      conv_act(acc[mt][nt][2 * hh + 1] + s_b2[co + 1], a2));
+                        if (t >= L) o = __floats2half2_rn(0.0f, 0.0f);  // beyond a short chunk's end: the next convolution's zero padding
+                        *reinterpret_cast<__half2*>(dst + co) = o;
+                    }
+                }
+            }
         }
-        parity ^= 1u;
     }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 4) tc::tmem_dealloc(tmem_acc, 32);
-}
-
-// ------------------------------------------------------------------------------------------------
-// LSTM layer for a hidden size whose weights fit one SM's tensor memory (fast: C = 96): all T steps of one layer in one
-// persistent launch, no inter-CTA traffic.
-//
-// Orientation is "weights as the M operand": per step, for each tile m of 32 hidden units,
-//     D_m[128 gate rows][16] = Wp_m[128][2C] * Z_t[16][2C]^T ,  Z_t = [x_t ; h_{t-1}]  (rows = chunks, zero-padded to 16)
-// where the 128 rows of Wp_m are (i | f | g | o) x 32 units, so one epilogue warp handles one gate type.  The permuted
-// weights (4C x 2C fp16) are written ONCE into tensor memory (tcgen05.st) and every MMA of the sequence reads its A operand
-// from there; the only shared-memory operand is the tiny Z_t: x_t arrives by TMA, h_t is written by the epilogue.
-//
-// A step is a dependent chain (MMA -> tcgen05.ld -> gates -> cell -> h_t -> MMA) of ~1000 cycles that leaves every pipe of
-// the SM idle most of the time, and a batch of 512 chunks only has 512 / NBR such chains.  So one CTA runs NG = 2 chains
-// ("groups") side by side: each group owns NBR chunks, its own Z / gate / cell buffers, barriers, accumulator columns and its
-// own 16 warps (1 TMA producer, MT MMA issuers, MT x 4 epilogue warps); the groups share nothing but the weights in tensor
-// memory, and one group's gate math runs under the other's MMAs and barrier hand-overs.
-// Accumulators are double-buffered per group so the x_t half of step s+1 (which does not depend on the recurrence) is
-// issued while the epilogue of step s still runs; only the h_{t-1} half sits on the critical path.
-// ------------------------------------------------------------------------------------------------
-constexpr int KBLK = 32;           // K elements per smem block (64 B rows, SWIZZLE_64B)
-constexpr int UN = 16;             // UMMA N: rows of a Z block (chunks, zero-padded when a group owns fewer)
-constexpr int ZBLK = UN * KBLK * 2;
-
-struct LstmParams {
-    __half* seq;        // [T][N][C] in place
-    const float* bias;  // [4C] permuted like the weight rows (b_ih + b_hh)
-    const __half* w;    // [4C][2C] permuted weights
-    int T, N, C, reverse;
-    long long* dbg;  // optional timeline (clock64 stamps of CTA 0 / group 0, steps 64..67); nullptr in production
-};
-
-__device__ __forceinline__ uint64_t umma_desc_sw64(uint32_t smem_addr) {
-    // K-major, rows of 64 B, 8-row groups 512 B apart, SWIZZLE_64B (layout type 4)
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3ffffu) >> 4);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(512 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)4 << 61;
-    return d;
-}
-
-__device__ __forceinline__ uint32_t sw64_offset(int row, int col) {
-    // byte offset of fp16 element (row, col<32) in a [rows x 32] SWIZZLE_64B tile
-    return (uint32_t)(row * 64 + ((((col >> 3) ^ ((row >> 1) & 3))) << 4) + ((col & 7) << 1));
 }
 
 // Gate activations on one MUFU.TANH each: sigmoid(v) = 0.5 tanh(0.5 v) + 0.5 (am = 1), tanh(v) (am = 2); FMUL, MUFU.TANH, FFMA.
-// A step of the recurrence applies 5 C activations per chunk, and with ex2 + rcp (two MUFU operations each, ~2^-22) the SFU
-// was the busiest unit of the fast kernel (44 % at 2 x 8 chunks per CTA) and capped how many chunks a CTA could carry:
-// 1.83 -> 1.60 ms per fast layer, 4.6 -> 4.1 ms per hac layer (profiles/r02_b19_*).  tanh.approx.f32 is good to ~2^-11 -- the
-// rounding h_t gets anyway when it is stored as fp16; score errors against both oracles are unchanged
-// (profiles/r02_b19_err_*.txt: the gates saturate and contract the error).  The same substitution in the swish of the
-// convolutions was rejected, see common.cuh.  -DB200_LSTM_EX2_RCP restores the two-MUFU form.
+// tanh.approx.f32 is good to ~2^-11 -- the rounding h_t gets anyway when it is stored as fp16, and the gates saturate and
+// contract the error.  The same substitution in the swish of the convolutions was rejected, see common.cuh.
+// -DB200_LSTM_EX2_RCP restores the two-MUFU form (ex2 + rcp).
 #ifndef B200_LSTM_EX2_RCP
 __device__ __forceinline__ float gate_act(float v, float am) {
     const float s = 0.5f * am;
@@ -364,562 +308,186 @@ __device__ __forceinline__ float gate_act(float v, float am) {
 #endif
 __device__ __forceinline__ float tanh_f(float v) { return gate_act(v, 2.0f); }
 
-// C   = hidden size (compile time so the MMA issue loops unroll into immediate-offset descriptors).
-// NBR = chunks owned by one group (2, 4, 8 or 16: small values spread a small batch over more SMs).
-// NG  = groups (independent recurrences) per CTA.
-template <int C, int NG>
-struct LstmCfg {
-    static constexpr int MT = C / 32;                 // gate tiles = MMA-issuing warps = epilogue warp quartets per group
-    static constexpr int KB = 2 * C / KBLK;
-    static constexpr int KBX = C / KBLK;
-    static constexpr int GROUP_WARPS = 1 + MT + 4 * MT;
-    static constexpr int THREADS = 32 * GROUP_WARPS * NG;
-    static constexpr int ACC_COLS = NG * 2 * MT * UN;
-    static constexpr int NEED_COLS = ACC_COLS + MT * C;   // + the weights: tile m, k-step ks at m*C + ks*8
-    static constexpr uint32_t TMEM_COLS = NEED_COLS <= 256 ? 256 : 512;
-    static constexpr int NBAR = 8 + 2 * MT;               // mbarriers per group
-    static_assert(NEED_COLS <= 512, "weights + accumulators must fit tensor memory");
-    static_assert(GROUP_WARPS % 4 == 0, "epilogue warps must keep warp % 4 == TMEM lane quarter");
-    static_assert(THREADS <= 1024 && NG * MT + 1 <= 16, "too many warps / named barriers");
-    static constexpr size_t smem_bytes(int nbr) {
-        return 1024 + (size_t)NG * (2 * KB * ZBLK + (size_t)MT * 4 * nbr * 32 * 4 + (size_t)MT * nbr * 32 * 4 + NBAR * 8) + 64;
-    }
-};
-
-template <int C, int NBR, int NG>
-__global__ void __launch_bounds__(LstmCfg<C, NG>::THREADS, 1) lstm_layer_kernel(const __grid_constant__ CUtensorMap tma_x,
-                                                                               const LstmParams p) {
-    using Cfg = LstmCfg<C, NG>;
-    constexpr int MT = Cfg::MT, KB = Cfg::KB, KBX = Cfg::KBX, GW = Cfg::GROUP_WARPS, NBAR = Cfg::NBAR;
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // realign by an integer offset from the __shared__ symbol so the compiler keeps the shared address space
-    uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int grp = warp / GW, lw = warp % GW;   // group and role within the group
-    uint8_t* z_all = smem;                                                        // [NG][2][KB][ZBLK]
-    float* g_all = reinterpret_cast<float*>(z_all + (size_t)NG * 2 * KB * ZBLK);  // [NG][MT][4][NBR][32]
-    float* c_all = g_all + (size_t)NG * MT * 4 * NBR * 32;                        // [NG][MT][NBR][32] cell state
-    uint64_t* bars_all = reinterpret_cast<uint64_t*>(c_all + (size_t)NG * MT * NBR * 32);
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars_all + NG * NBAR);
-    uint8_t* z_s = z_all + (size_t)grp * 2 * KB * ZBLK;
-    float* c_s = c_all + (size_t)grp * MT * NBR * 32;
-    uint64_t* bars = bars_all + grp * NBAR;
-    uint64_t* x_full = bars;          // [2]  TMA -> MMA
-    uint64_t* z_free = bars + 2;      // [2]  MMAs done with Z[buf] -> TMA
-    uint64_t* h_ready = bars + 4;     // [2]  epilogue wrote h into Z[buf] -> MMA
-    uint64_t* acc_free = bars + 6;    // [2]  epilogue done reading accumulator set -> MMA
-    uint64_t* acc_full = bars + 8;    // [2][MT] MMA -> epilogue
-    const int n0 = (blockIdx.x * NG + grp) * NBR;
-
-    // zero Z (padding rows, h_{-1}) and the cell state before anything asynchronous starts
-    for (int i = threadIdx.x; i < NG * 2 * KB * ZBLK / 16; i += blockDim.x) reinterpret_cast<uint4*>(z_all)[i] = make_uint4(0, 0, 0, 0);
-    for (int i = threadIdx.x; i < NG * MT * NBR * 32; i += blockDim.x) c_all[i] = 0.0f;
-    tc::fence_proxy_async_smem();
-    if (threadIdx.x == 0) {
-        for (int gi = 0; gi < NG; ++gi) {
-            uint64_t* b = bars_all + gi * NBAR;
-            for (int i = 0; i < 2; ++i) {
-                tc::mbar_init(&b[i], 1);
-                tc::mbar_init(&b[2 + i], MT);        // one commit per MMA-issuing warp
-                tc::mbar_init(&b[4 + i], MT * 4);    // one arrival per epilogue warp
-                tc::mbar_init(&b[6 + i], MT * 4);
-            }
-            for (int i = 0; i < 2 * MT; ++i) tc::mbar_init(&b[8 + i], 1);
-        }
-        tc::fence_barrier_init();
-        tc::prefetch_tmap(&tma_x);
-    }
-    if (warp == 1) tc::tmem_alloc(tmem_holder, Cfg::TMEM_COLS);
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_base = *tmem_holder;
-    const uint32_t tmem_acc = tmem_base + (uint32_t)(grp * 2 * MT * UN);
-    const uint32_t tmem_w = tmem_base + Cfg::ACC_COLS;
-    if (grp == 0 && lw > MT) {
-        // weights into tensor memory: epilogue warp (tile m, lane quarter q) of group 0, one weight row per thread
-        const int m = (lw - (1 + MT)) >> 2, q = warp & 3;
-        const uint4* src = reinterpret_cast<const uint4*>(p.w + (size_t)(m * 128 + q * 32 + lane) * 2 * C);
-#pragma unroll 1
-        for (int cb = 0; cb < C / 32; ++cb) {
-            uint32_t r[32];
-#pragma unroll
-            for (int v = 0; v < 8; ++v) {
-                const uint4 x = __ldg(src + cb * 8 + v);
-                r[4 * v] = x.x; r[4 * v + 1] = x.y; r[4 * v + 2] = x.z; r[4 * v + 3] = x.w;
-            }
-            tc::tmem_st_32x32(tmem_w + ((uint32_t)(q * 32) << 16) + (uint32_t)(m * C + cb * 32), r);
-        }
-        tc::tmem_st_wait();
-    }
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::tc_fence_after();
-
-    if (lw == 0) {
-        // ---------------- TMA producer ----------------
-        if (tc::elect_one()) {
-            for (int s = 0; s < p.T; ++s) {
-                const int t = p.reverse ? p.T - 1 - s : s;
-                const int buf = s & 1;
-                tc::mbar_wait(&z_free[buf], ((s >> 1) & 1) ^ 1);
-                tc::mbar_arrive_expect_tx(&x_full[buf], (uint32_t)(KBX * NBR * KBLK * 2));
-                for (int kb = 0; kb < KBX; ++kb) {
-                    tc::tma_load_2d(z_s + (size_t)(buf * KB + kb) * ZBLK, &tma_x, &x_full[buf], kb * KBLK, t * p.N + n0);
-                }
-            }
-        }
-    } else if (lw <= MT) {
-        // ---------------- MMA issuers: warp m issues the MMAs of gate tile m ----------------
-        const int m = lw - 1;
-        if (tc::elect_one()) {
-            constexpr uint32_t idesc = tc::umma_idesc_f16(128, UN);
-            const uint64_t zdesc0 = umma_desc_sw64(tc::smem_u32(z_s));
-            for (int s = 0; s < p.T; ++s) {
-                const int buf = s & 1;
-                const uint32_t par = (uint32_t)((s >> 1) & 1);
-                const uint64_t zd = zdesc0 + (uint64_t)((buf * KB * ZBLK) >> 4);
-                const uint32_t d_tmem = tmem_acc + (uint32_t)((buf * MT + m) * UN);
-                const bool dbg = p.dbg && blockIdx.x == 0 && warp == 1 && s >= 64 && s < 68;
-                tc::mbar_wait(&x_full[buf], par);
-                tc::mbar_wait(&acc_free[buf], par ^ 1);
-                tc::tc_fence_after();
-#pragma unroll
-                for (int half = 0; half < 2; ++half) {
-                    if (half == 1) {
-                        if (dbg) p.dbg[(s - 64) * 16 + 0] = clock64();
-                        tc::mbar_wait(&h_ready[buf], par);
-                        tc::tc_fence_after();
-                        if (dbg) p.dbg[(s - 64) * 16 + 1] = clock64();
-                    }
-#pragma unroll
-                    for (int kb = half * KBX; kb < (half + 1) * KBX; ++kb) {
-                        const uint64_t bdesc = zd + (uint64_t)((kb * ZBLK) >> 4);
-                        const uint32_t a_t = tmem_w + (uint32_t)(m * C + kb * 16);  // 16 columns per 32-element block
-                        tc::umma_f16_ts(d_tmem, a_t, bdesc, idesc, kb != 0);
-                        tc::umma_f16_ts(d_tmem, a_t + 8, bdesc + 2, idesc, true);
-                    }
-                }
-                tc::umma_commit(&acc_full[buf * MT + m]);
-                tc::umma_commit(&z_free[buf]);
-                if (dbg) p.dbg[(s - 64) * 16 + 2] = clock64();
-            }
-        }
-    } else {
-        // ---------------- epilogue quartets: gates, cell update, h_t ----------------
-        const int ewarp = lw - (1 + MT);
-        const int m = ewarp >> 2;    // gate tile
-        const int ew = ewarp & 3;    // warp within the quartet -> chunks ew, ew + 4, ...
-        const int gate = warp & 3;   // TMEM lane quarter this warp may read == gate type (i,f,g,o)
-        const int bar_id = 1 + grp * MT + m;
-        float* gs = g_all + ((size_t)grp * MT + m) * 4 * NBR * 32;
-        constexpr int CPT = (NBR + 3) / 4;
-        const float b = __ldg(p.bias + m * 128 + gate * 32 + lane);
-        const float am = gate == 2 ? 2.0f : 1.0f;  // tanh(v) = 1 - 2/(e^{2v}+1), sigmoid(v) = 1 - 1/(e^{v}+1)
-        if (lane == 0) tc::mbar_arrive(&h_ready[0]);  // h_{-1} = 0 is in place (zeroed before the CTA-wide sync)
-
-        for (int s = 0; s < p.T; ++s) {
-            const int t = p.reverse ? p.T - 1 - s : s;
-            const int buf = s & 1, nbuf = buf ^ 1;
-            const uint32_t par = (uint32_t)((s >> 1) & 1);
-            uint8_t* zh_next = z_s + (size_t)(nbuf * KB + KBX) * ZBLK;
-            __half* y_t = p.seq + ((size_t)t * p.N + n0) * C;
-            const bool dbg = p.dbg && blockIdx.x == 0 && grp == 0 && ewarp == 0 && lane == 0 && s >= 64 && s < 68;
-            if (dbg) p.dbg[(s - 64) * 16 + 4] = clock64();
-            tc::mbar_wait(&acc_full[buf * MT + m], par);
-            tc::tc_fence_after();
-            if (dbg) p.dbg[(s - 64) * 16 + 5] = clock64();
-            uint32_t r[NBR];
-            const uint32_t taddr = tmem_acc + ((uint32_t)(gate * 32) << 16) + (uint32_t)((buf * MT + m) * UN);
-            if constexpr (NBR == 16) {
-                tc::tmem_ld_32x16(taddr, r);
-            } else if constexpr (NBR == 8) {
-                tc::tmem_ld_32x8(taddr, r);
-            } else if constexpr (NBR == 4) {
-                tc::tmem_ld_32x4(taddr, r);
-            } else {
-                tc::tmem_ld_32x2(taddr, r);
-            }
-            tc::tmem_ld_wait();
-            if (dbg) p.dbg[(s - 64) * 16 + 6] = clock64();
-#pragma unroll
-            for (int n = 0; n < NBR; ++n) gs[(gate * NBR + n) * 32 + lane] = gate_act(__uint_as_float(r[n]) + b, am);
-            float c_old[CPT];
-#pragma unroll
-            for (int j = 0; j < CPT; ++j) {
-                const int n = ew + 4 * j;
-                c_old[j] = n < NBR ? c_s[((size_t)m * NBR + n) * 32 + lane] : 0.0f;
-            }
-            if (dbg) p.dbg[(s - 64) * 16 + 7] = clock64();
-            named_bar_sync(bar_id, 128);
-            if (dbg) p.dbg[(s - 64) * 16 + 8] = clock64();
-#pragma unroll
-            for (int j = 0; j < CPT; ++j) {
-                const int n = ew + 4 * j;
-                if (n < NBR) {
-                    const float ig = gs[(0 * NBR + n) * 32 + lane];
-                    const float fg = gs[(1 * NBR + n) * 32 + lane];
-                    const float gg = gs[(2 * NBR + n) * 32 + lane];
-                    const float og = gs[(3 * NBR + n) * 32 + lane];
-                    const float cs = fg * c_old[j] + ig * gg;
-                    c_s[((size_t)m * NBR + n) * 32 + lane] = cs;  // owned by this thread for all steps
-                    const __half h = __float2half_rn(og * tanh_f(cs));
-                    *reinterpret_cast<__half*>(zh_next + (size_t)m * ZBLK + sw64_offset(n, lane)) = h;
-                    y_t[(size_t)n * C + m * 32 + lane] = h;
-                }
-            }
-            if (dbg) p.dbg[(s - 64) * 16 + 9] = clock64();
-            tc::tc_fence_before();
-            tc::fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) {
-                tc::mbar_arrive(&acc_free[buf]);
-                tc::mbar_arrive(&h_ready[nbuf]);
-            }
-            if (dbg) p.dbg[(s - 64) * 16 + 10] = clock64();
-            named_bar_sync(bar_id, 128);  // gs reuse across steps
-        }
-    }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tc::tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-}
-
 // ------------------------------------------------------------------------------------------------
-// LSTM layer for hidden sizes whose weights do not fit one SM (hac: C = 384): hoisted x-projection + cluster recurrence.
+// LSTM layer = hoisted x-projection + recurrence.
 //
-// The x_t half of the gate pre-activations does not depend on the recurrence, so it is hoisted into one large
-// tcgen05 GEMM per layer (gemm.cu) that writes gx[t][chunk block of 32][gate row][chunk] (fp16, bias included).  Gate rows
-// are permuted so that a warp's 32 TMEM lanes hold (8 units x 4 gates).
+// The x_t half of the gate pre-activations does not depend on the recurrence, so it is one large wgmma GEMM per layer
+// (gemm.cu) that writes gx[t][chunk][4C] (fp16, b_ih + b_hh included, PyTorch gate order i | f | g | o).
 //
-// Recurrence: W_hh (4C x C fp16 = 1.18 MB for C = 384) is split by gate tile across the CL = 6 CTAs of a thread-block
-// cluster and stays in their TENSOR MEMORY for the whole sequence (A operand of tcgen05.mma read from TMEM, written once with
-// tcgen05.st).  Every step each CTA computes the gates of its own 32 * TPC hidden units from the full h_{t-1} (its private
-// copy in shared memory) and all-gathers its slice of h_t into every CTA's copy.  The kernel is built around what bounds a
-// step -- the latency of that exchange and of the gate math -- not around barriers:
-//   * the cluster's chunks form NG = 2 independent groups of GN = 16 or 32; the MMA issuer ping-pongs between them, so group
-//     A's gate math and all-gather run under group B's MMAs (a single group has nothing to overlap with);
-//   * h_t travels as BULK ASYNC COPIES (cp.async.bulk shared::cta -> shared::cluster): an epilogue tile stages its
-//     32 units x GN chunks in the swizzled operand layout in local shared memory and one thread sends the block to
-//     every CTA of the cluster; the bytes complete on the destination's mbarrier, which is what its MMA issuer waits on.
-//     No cluster barrier, no remote scalar stores, and the operand is written and read by the async proxy (no
-//     generic->async fence on the receiving side).  Measured alternatives, both slower (3.3 -> 5.7 ms per layer,
-//     profiles/r02_b3_*, r02_b5_*): the exchange through L2 (TMA store + multicast TMA load) and remote 16-byte stores with
-//     remote mbarrier arrivals;
-//   * the same staged block leaves for HBM as one TMA store (no per-thread global stores);
-//   * the four gates of a cell meet by quad transposes in registers (shuffles) instead of a shared-memory exchange.
-// A step's cost hardly depends on GN (it is latency, ~12 small copies per CTA and group), so GN = 32 -- 64 chunks per
-// cluster, 8 clusters = 48 SMs for a batch of 512 -- does the same work in fewer SM-cycles and leaves room for the
-// recurrences of two more batches next to it; GN = 16 is the lower-latency shape for a lone runner.
-// Safety of buffer reuse without extra barriers (Z and staging are double-buffered): a CTA starts step s+2 for a group
-// only after every CTA's slice of h_{s+1} has landed, which those CTAs sent only after their step-(s+1) MMAs completed,
-// which needed every slice of h_s to have landed everywhere -- so by then nobody reads Z[(s) & 1] of step s or the
-// staging block sent at step s any more.
+// Recurrence (lstm_rec_kernel): a thread-block cluster of CL CTAs owns NB chunks; CTA `rank` owns hidden units
+// [rank * U, rank * U + U), U = C / CL, i.e. 4U gate rows of W_hh.  Those rows live in REGISTERS for the whole sequence, as
+// mma.sync A fragments: warp w holds gate rows 16 w .. 16 w + 15 for all of K = C (C / 16 x 4 registers per thread).  A
+// step is
+//     G[4U][NB] = W_hh[rows of this CTA] h_{t-1}      mma.sync m16n8k16, B fragments by ldmatrix from this CTA's copy of h
+//     gates, cell update, h_t (fp16)                    thread = a pair of adjacent units x one chunk, cell state in registers
+//     h_t -> every CTA's copy of h (distributed shared memory) and to the sequence buffer, one cluster barrier
+// The step is a latency chain (MMA -> barrier -> gate math -> all-gather -> barrier) rather than a throughput problem:
+// mma.sync on register-resident weights keeps that chain short, where wgmma would add its asynchronous hand-offs and a
+// 64-row granularity to every step.  h is double-buffered, so one cluster barrier per step orders both the all-gather of
+// h_t before the MMAs of step t+1 and the reads of h_{t-1} before its buffer is overwritten at step t+1.
+// C = 96 runs as a cluster of one CTA (all 384 gate rows in one CTA); C = 192 and 384 split over 4 and 8 CTAs.
 // ------------------------------------------------------------------------------------------------
 struct LstmRecParams {
-    __half* seq;          // [T][N][C] output h (in place over the layer input)
-    const __half* gx;     // [T][N / 32][4C][32]
+    __half* seq;          // [T][N][C] output h (in place over the layer input, which gx has consumed)
+    const __half* gx;     // [T][N][4C]
+    const __half* w_hh;   // [4C][C], PyTorch row order
     int T, N, reverse;
     const int32_t* lens;  // optional per-chunk length in samples (variable chunk sizes); stride = samples per step
     int stride;
-    long long* dbg;       // optional clock64 timeline of CTA 0, steps 64..67 (B200_DEBUG_LSTM_TIMELINE); nullptr in production
 };
 
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t local_addr, uint32_t cta_rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(cta_rank));
-    return r;
-}
-__device__ __forceinline__ void cluster_arrive_release() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
-__device__ __forceinline__ void cluster_wait_acquire() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
+// CTAs per cluster for a hidden size: the CTA's W_hh rows (4 C / CL x C fp16) must fit its registers
+__host__ __device__ constexpr int rec_cluster(int C) { return C <= 96 ? 1 : C <= 192 ? 4 : 8; }
 
-template <int C, int CL, int NG, int GN>
-struct ClusterCfg {
-    static constexpr int MT = C / 32;
-    static constexpr int TPC = MT / CL;            // gate tiles per CTA
-    static constexpr int KBH = C / KBLK;           // operand blocks (32 hidden units each)
-    static constexpr int UNC = NG * GN;            // chunks per cluster
-    static constexpr int NQ = GN / 4;              // chunk quads per group: a lane owns the cells (unit, chunk 4c + gate lane)
-    static constexpr int EW = 4 * TPC * NG;        // epilogue warps: (group, tile, TMEM lane quarter)
-    static constexpr int THREADS = 64 + 32 * EW;
-    static constexpr int ZB = GN * KBLK * 2;       // bytes of one operand block (GN chunk rows x 32 fp16)
-    static constexpr int WCOLS = C / 2;            // TMEM columns of one weight tile
-    static constexpr int ACC0 = TPC * WCOLS;       // accumulators start behind the weights
-    static constexpr int NEED = ACC0 + NG * TPC * GN;
-    static constexpr uint32_t TMEM_COLS = NEED <= 64 ? 64 : NEED <= 128 ? 128 : NEED <= 256 ? 256 : 512;
-    static constexpr size_t Z_BYTES = (size_t)NG * 2 * KBH * ZB;      // [group][buffer][block]
-    static constexpr size_t ST_BYTES = (size_t)NG * 2 * TPC * ZB;     // [group][buffer][tile] staging
-    static constexpr size_t SMEM = 1024 + Z_BYTES + ST_BYTES + 1024;
-    static_assert(MT % CL == 0 && NEED <= 512, "tile split / tensor memory budget");
-    static_assert(GN == 16 || GN == 32, "a group is 16 or 32 chunks (UMMA N, tcgen05.ld shape, gx block)");
-    static_assert(UNC <= 64, "chunk-length table");
+template <int C, int CL, int NB>
+struct RecCfg {
+    static constexpr int U = C / CL;              // hidden units per CTA
+    static constexpr int MT = 4 * U / 16;         // m16 tiles of gate rows = warps
+    static constexpr int THREADS = 32 * MT;
+    static constexpr int KS = C / 16;             // K steps
+    static constexpr int NT = NB / 8;             // n8 tiles of chunks
+    static constexpr int HS = C + 8;              // row stride of h (fp16): the 8 rows of an ldmatrix phase on distinct banks
+    static constexpr int GS = NB + 4;             // row stride of the gate pre-activations (fp32)
+    static constexpr int PAIRS = U / 2 * NB / THREADS;   // (unit pair, chunk) cells per thread
+    // gx is loaded ahead of the MMAs when it fits the registers; with 4 cell pairs per thread (64 chunks per cluster) the
+    // 16 extra registers would spill, so gx is loaded in the cell loop instead
+    static constexpr bool GX_AHEAD = PAIRS <= 2;
+    static constexpr size_t SMEM = (size_t)2 * NB * HS * 2 + (size_t)4 * U * GS * 4;
+    static_assert(C % CL == 0 && U % 4 == 0 && NT % 2 == 0 && PAIRS >= 1 && (U / 2 * NB) % THREADS == 0, "recurrence shape");
+    static_assert(THREADS <= 1024 && CL <= 8, "block / cluster size");
 };
 
-template <int C, int CL, int NG, int GN>
-__global__ void __launch_bounds__(ClusterCfg<C, CL, NG, GN>::THREADS, 1) lstm_cluster_kernel(const __grid_constant__ CUtensorMap tma_y,
-                                                                                            const __half* __restrict__ w_hh,
-                                                                                            const LstmRecParams p) {
-    using Cfg = ClusterCfg<C, CL, NG, GN>;
-    constexpr int TPC = Cfg::TPC, KBH = Cfg::KBH, ZB = Cfg::ZB, NQ = Cfg::NQ;
-    constexpr int GB = 32;  // chunk block of the gx layout
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* z_s = smem;                                   // [NG][2][KBH][ZB]  this CTA's copy of the full h
-    uint8_t* st_s = z_s + Cfg::Z_BYTES;                    // [NG][2][TPC][ZB]  h_t of this CTA's units, staged for sending
-    uint64_t* bars = reinterpret_cast<uint64_t*>(st_s + Cfg::ST_BYTES);
-    uint64_t* h_full = bars;                               // [NG][2]   bytes of h landed -> MMA issuer
-    uint64_t* acc_full = bars + NG * 2;                    // [NG][TPC] MMA -> epilogue
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(acc_full + NG * TPC);
-    int* len_s = reinterpret_cast<int*>(tmem_holder + 2);   // [UNC] steps of every chunk of the cluster (variable chunk sizes)
-
+template <int C, int CL, int NB>
+__global__ void __launch_bounds__(RecCfg<C, CL, NB>::THREADS, 1) lstm_rec_kernel(const LstmRecParams p) {
+    using Cfg = RecCfg<C, CL, NB>;
+    constexpr int U = Cfg::U, KS = Cfg::KS, NT = Cfg::NT, HS = Cfg::HS, GS = Cfg::GS, PAIRS = Cfg::PAIRS;
+    constexpr bool GX_AHEAD = Cfg::GX_AHEAD;
+    extern __shared__ __align__(16) uint8_t smem_raw[];
+    __half* h_s = reinterpret_cast<__half*>(smem_raw);                      // [2][NB][HS]  this CTA's copy of h
+    float* g_s = reinterpret_cast<float*>(smem_raw + (size_t)2 * NB * HS * 2);  // [4U][GS]
+    __shared__ int len_s[NB];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const int cluster_id = blockIdx.x / CL;
-    const int n0 = cluster_id * Cfg::UNC;
-    if (threadIdx.x < Cfg::UNC) {
-        len_s[threadIdx.x] = p.lens ? min(p.T, __ldg(p.lens + n0 + threadIdx.x) / p.stride) : p.T;
-    }
+    cg::cluster_group cluster = cg::this_cluster();
+    const int rank = CL > 1 ? (int)cluster.block_rank() : 0;
+    const int n0 = (int)(blockIdx.x / CL) * NB;
+    if (threadIdx.x < NB) len_s[threadIdx.x] = p.lens ? min(p.T, __ldg(p.lens + n0 + threadIdx.x) / p.stride) : p.T;
+    for (int i = threadIdx.x; i < 2 * NB * HS / 8; i += Cfg::THREADS) reinterpret_cast<uint4*>(h_s)[i] = make_uint4(0, 0, 0, 0);
 
-    for (int i = threadIdx.x; i < (int)((Cfg::Z_BYTES + Cfg::ST_BYTES) / 16); i += blockDim.x) {
-        reinterpret_cast<uint4*>(z_s)[i] = make_uint4(0, 0, 0, 0);
-    }
-    tc::fence_proxy_async_smem();
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < NG * 2; ++i) tc::mbar_init(&h_full[i], 1);   // one armed arrival + the bytes of all slices
-        for (int i = 0; i < NG * TPC; ++i) tc::mbar_init(&acc_full[i], 1);
-        tc::fence_barrier_init();
-        tc::prefetch_tmap(&tma_y);
-    }
-    if (warp == 1) tc::tmem_alloc(tmem_holder, Cfg::TMEM_COLS);
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_base = *tmem_holder;
-
-    const bool is_epi = warp >= 2;
-    const int ew = warp - 2;
-    const int eg = ew / (4 * TPC);        // group served by this epilogue warp
-    const int ti = (ew >> 2) % TPC;       // tile of this CTA
-    const int qt = warp & 3;              // TMEM lane quarter (the 4 warps of a (group, tile) cover all four)
-    if (is_epi && eg == 0) {
-        // this thread's weight row (tile rank*TPC + ti, row 32*qt + lane) -> tensor memory, once
-        const int m = (int)rank * TPC + ti;
-        const uint4* src = reinterpret_cast<const uint4*>(w_hh + (size_t)(m * 128 + qt * 32 + lane) * C);
-#pragma unroll 1
-        for (int cb = 0; cb < C / 64; ++cb) {
-            uint32_t r[32];
+    // A fragments: local gate row r <-> W_hh row (r / U) * C + rank * U + r % U
+    uint32_t a[KS][4];
+    {
+        const int r_lo = warp * 16 + (lane >> 2), r_hi = r_lo + 8;
+        const __half* w_lo = p.w_hh + (size_t)((r_lo / U) * C + rank * U + r_lo % U) * C;
+        const __half* w_hi = p.w_hh + (size_t)((r_hi / U) * C + rank * U + r_hi % U) * C;
 #pragma unroll
-            for (int v = 0; v < 8; ++v) {
-                const uint4 x = __ldg(src + cb * 8 + v);
-                r[4 * v] = x.x; r[4 * v + 1] = x.y; r[4 * v + 2] = x.z; r[4 * v + 3] = x.w;
-            }
-            tc::tmem_st_32x32(tmem_base + ((uint32_t)(qt * 32) << 16) + (uint32_t)(ti * Cfg::WCOLS + cb * 32), r);
+        for (int ks = 0; ks < KS; ++ks) {
+            const int col = ks * 16 + 2 * (lane & 3);
+            a[ks][0] = __ldg(reinterpret_cast<const unsigned int*>(w_lo + col));
+            a[ks][1] = __ldg(reinterpret_cast<const unsigned int*>(w_hi + col));
+            a[ks][2] = __ldg(reinterpret_cast<const unsigned int*>(w_lo + col + 8));
+            a[ks][3] = __ldg(reinterpret_cast<const unsigned int*>(w_hi + col + 8));
         }
-        tc::tmem_st_wait();
     }
-    if (threadIdx.x == 0) {
-        // h_{-1} = 0 is in place: complete phase 0 of the buffer-0 barriers without bytes
-        for (int g = 0; g < NG; ++g) tc::mbar_arrive(&h_full[g * 2 + 0]);
-    }
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::tc_fence_after();
-    // every CTA of the cluster has zeroed its operand buffers and initialised its barriers before any remote copy lands
-    cluster_arrive_release();
-    cluster_wait_acquire();
+    // cells: pair index q = threadIdx.x + j * THREADS -> units (u, u + 1), u = 2 (q % (U / 2)), chunk q / (U / 2)
+    float c_reg[PAIRS][2];
+#pragma unroll
+    for (int j = 0; j < PAIRS; ++j) c_reg[j][0] = c_reg[j][1] = 0.0f;
+    // every CTA of the cluster has zeroed its copy of h before anybody writes h_0 into it
+    if constexpr (CL > 1) cluster.sync();
+    else __syncthreads();
 
-    const uint32_t z_local = tc::smem_u32(z_s);
-    // A chunk shorter than the batch's chunk size is the sequence 0 .. len-1: outside it the state is zero (masked in the
-    // epilogue), so the cluster only walks the steps some chunk of it is alive in -- the last ones backwards, the first
-    // ones forwards -- and short chunks grouped in a cluster cost proportionally less.
     int steps = 0;
-#pragma unroll 4
-    for (int i = 0; i < Cfg::UNC; ++i) steps = max(steps, len_s[i]);
-    if (warp == 1) {
-        // ---------------- MMA issuer ----------------
-        if (tc::elect_one()) {
-            const uint64_t zdesc0 = umma_desc_sw64(z_local);
-            constexpr uint32_t idesc = tc::umma_idesc_f16(128, GN);
-            for (int s = 0; s < steps; ++s) {
-                const int buf = s & 1, nbuf = buf ^ 1;
-                const uint32_t par = (uint32_t)((s >> 1) & 1);
+    for (int i = 0; i < NB; ++i) steps = max(steps, len_s[i]);
+    const int qm = lane >> 3, qr = lane & 7;   // ldmatrix: matrix qm = (n tile qm / 2, k half qm % 2), row qr
+    for (int s = 0; s < steps; ++s) {
+        const int t = p.reverse ? steps - 1 - s : s;
+        const int cur = s & 1, nxt = cur ^ 1;
+        // gx of this thread's cells: independent of the recurrence, in flight while the MMAs run (GX_AHEAD)
+        auto load_gx = [&](int j, __half2* dst) {
+            const int q = threadIdx.x + j * Cfg::THREADS;
+            const int u = 2 * (q % (U / 2)), n = q / (U / 2);
+            const __half* gp = p.gx + ((size_t)t * p.N + n0 + n) * (4 * C) + rank * U + u;
 #pragma unroll
-                for (int g = 0; g < NG; ++g) {
-                    // arm the barrier the slices of h_s will complete on (all CL CTAs x TPC tiles, this group)
-                    if (s + 1 < steps) tc::mbar_arrive_expect_tx(&h_full[g * 2 + nbuf], (uint32_t)(CL * TPC * ZB));
-                    long long* d = (p.dbg && blockIdx.x == 0 && s >= 64 && s < 68) ? p.dbg + (s - 64) * 32 + g * 4 : nullptr;
-                    if (d) d[0] = clock64();
-                    tc::mbar_wait(&h_full[g * 2 + buf], par);
-                    tc::tc_fence_after();
-                    if (d) d[1] = clock64();
-                    const uint64_t zd = zdesc0 + (uint64_t)(((g * 2 + buf) * KBH * ZB) >> 4);
+            for (int g = 0; g < 4; ++g) dst[g] = *reinterpret_cast<const __half2*>(gp + g * C);
+        };
+        __half2 gxv[GX_AHEAD ? PAIRS : 1][4];
+        if constexpr (GX_AHEAD) {
 #pragma unroll
-                    for (int i = 0; i < TPC; ++i) {
-                        const uint32_t d_tmem = tmem_base + (uint32_t)(Cfg::ACC0 + (g * TPC + i) * GN);
+            for (int j = 0; j < PAIRS; ++j) load_gx(j, gxv[j]);
+        }
+        float acc[NT][4];
 #pragma unroll
-                        for (int kb = 0; kb < KBH; ++kb) {
-                            const uint32_t a_t = tmem_base + (uint32_t)(i * Cfg::WCOLS + kb * 16);
-                            const uint64_t bdesc = zd + (uint64_t)((kb * ZB) >> 4);
-                            tc::umma_f16_ts(d_tmem, a_t, bdesc, idesc, kb != 0);
-                            tc::umma_f16_ts(d_tmem, a_t + 8, bdesc + 2, idesc, true);
-                        }
-                        tc::umma_commit(&acc_full[g * TPC + i]);
-                    }
-                    if (d) d[2] = clock64();
-                }
+        for (int nt = 0; nt < NT; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.0f;
+        const uint32_t hb = tc::smem_u32(h_s + cur * NB * HS);
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+#pragma unroll
+            for (int np = 0; np < NT / 2; ++np) {
+                uint32_t b[4];
+                const int n = (2 * np + (qm >> 1)) * 8 + qr, k = ks * 16 + (qm & 1) * 8;
+                tc::ldmatrix_x4(b, hb + (uint32_t)((n * HS + k) * 2));
+                tc::mma_f16_16816(acc[2 * np], a[ks], b[0], b[1]);
+                tc::mma_f16_16816(acc[2 * np + 1], a[ks], b[2], b[3]);
             }
         }
-        __syncwarp();
-    } else if (is_epi) {
-        // ---------------- epilogue: gates, cell update, h_t out ----------------
-        const int uk = lane >> 2, gj = lane & 3;   // unit within the warp's 8, gate type (i, f, g, o)
-        const int g0 = gj & 1, g1 = gj >> 1;
-        const int m = (int)rank * TPC + ti;        // global tile = operand block this warp's units belong to
-        const float am = gj == 2 ? 2.0f : 1.0f;    // tanh(v) = 1 - 2/(e^{2v}+1), sigmoid(v) = 1 - 1/(e^{v}+1)
-        const bool sender = qt == 0 && lane == 0;
-        const int bar_id = 1 + eg * TPC + ti;
-        float c_reg[NQ];                           // cells (unit uk, chunk 4c + gj)
+        {
+            const int r_lo = warp * 16 + (lane >> 2);
 #pragma unroll
-        for (int c = 0; c < NQ; ++c) c_reg[c] = 0.0f;
-        const uint32_t taddr = tmem_base + ((uint32_t)(qt * 32) << 16) + (uint32_t)(Cfg::ACC0 + (eg * TPC + ti) * GN);
-        const int nc0 = n0 + eg * GN;              // first chunk of this group
-        const size_t gx_step = (size_t)(p.N / GB) * (size_t)(4 * C) * GB;
-        const __half* gx_base = p.gx + (size_t)(nc0 / GB) * (size_t)(4 * C) * GB + (size_t)(m * 128 + qt * 32 + lane) * GB + (size_t)(nc0 % GB);
-        // remote addresses of this tile's operand block and of the barrier it completes on, per buffer
-        uint32_t dst_z[2], dst_bar[2];
-#pragma unroll
-        for (int b = 0; b < 2; ++b) {
-            dst_z[b] = z_local + (uint32_t)(((eg * 2 + b) * KBH + m) * ZB);
-            dst_bar[b] = tc::smem_u32(&h_full[eg * 2 + b]);
+            for (int nt = 0; nt < NT; ++nt) {
+                const int col = nt * 8 + 2 * (lane & 3);
+                *reinterpret_cast<float2*>(g_s + r_lo * GS + col) = make_float2(acc[nt][0], acc[nt][1]);
+                *reinterpret_cast<float2*>(g_s + (r_lo + 8) * GS + col) = make_float2(acc[nt][2], acc[nt][3]);
+            }
         }
-        int my_len[NQ];   // steps of the chunks this lane owns cells of
+        __syncthreads();
 #pragma unroll
-        for (int c = 0; c < NQ; ++c) my_len[c] = len_s[eg * GN + 4 * c + gj];
-        for (int s = 0; s < steps; ++s) {
-            const int t = p.reverse ? steps - 1 - s : s;
-            const int nbuf = (s & 1) ^ 1;
-            const uint4* gp = reinterpret_cast<const uint4*>(gx_base + (size_t)t * gx_step);
-            uint4 gxv[GN / 8];
+        for (int j = 0; j < PAIRS; ++j) {
+            const int q = threadIdx.x + j * Cfg::THREADS;
+            const int u = 2 * (q % (U / 2)), n = q / (U / 2);
+            // outside the chunk (variable chunk sizes) the state is held at zero: a multiplicative mask, not a branch
+            const float alive = t < len_s[n] ? 1.0f : 0.0f;
+            __half2 gxl[4];
+            const __half2* gxj = gxl;
+            if constexpr (GX_AHEAD) gxj = gxv[j];
+            else load_gx(j, gxl);
+            float hv[2];
 #pragma unroll
-            for (int e = 0; e < GN / 8; ++e) gxv[e] = __ldg(gp + e);
-            uint8_t* stage = st_s + (size_t)((eg * 2 + (s & 1)) * TPC + ti) * ZB;
-            long long* d = (p.dbg && blockIdx.x == 0 && ew == 0 && lane == 0 && s >= 64 && s < 68) ? p.dbg + (s - 64) * 32 + 8 : nullptr;
-            if (d) d[0] = clock64();
-            tc::mbar_wait(&acc_full[eg * TPC + ti], (uint32_t)(s & 1));
-            tc::tc_fence_after();
-            if (d) d[1] = clock64();
-            uint32_t r[GN];
-            if constexpr (GN == 32) {
-                tc::tmem_ld_32x32(taddr, r);
+            for (int e = 0; e < 2; ++e) {
+                float pre[4];
+#pragma unroll
+                for (int g = 0; g < 4; ++g) {
+                    const float2 x = __half22float2(gxj[g]);
+                    pre[g] = g_s[(g * U + u + e) * GS + n] + (e ? x.y : x.x);
+                }
+                const float ig = gate_act(pre[0], 1.0f), fg = gate_act(pre[1], 1.0f);
+                const float gg = gate_act(pre[2], 2.0f), og = gate_act(pre[3], 1.0f);
+                const float cs = (fg * c_reg[j][e] + ig * gg) * alive;
+                c_reg[j][e] = cs;
+                hv[e] = og * tanh_f(cs) * alive;
+            }
+            const __half2 h2 = __floats2half2_rn(hv[0], hv[1]);
+            *reinterpret_cast<__half2*>(p.seq + ((size_t)t * p.N + n0 + n) * C + rank * U + u) = h2;
+            __half* h_own = h_s + (nxt * NB + n) * HS + rank * U + u;
+            if constexpr (CL > 1) {
+#pragma unroll
+                for (int r = 0; r < CL; ++r) *reinterpret_cast<__half2*>(cluster.map_shared_rank(h_own, r)) = h2;
             } else {
-                tc::tmem_ld_32x16(taddr, r);
+                *reinterpret_cast<__half2*>(h_own) = h2;
             }
-            tc::tmem_ld_wait();
-            tc::tc_fence_before();
-            if (d) d[2] = clock64();
-            float a[GN];
-#pragma unroll
-            for (int e = 0; e < GN / 8; ++e) {
-                const __half2* hx = reinterpret_cast<const __half2*>(&gxv[e]);
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const float2 f = __half22float2(hx[j]);
-                    a[8 * e + 2 * j] = gate_act(__uint_as_float(r[8 * e + 2 * j]) + f.x, am);
-                    a[8 * e + 2 * j + 1] = gate_act(__uint_as_float(r[8 * e + 2 * j + 1]) + f.y, am);
-                }
-            }
-            if (d) d[3] = clock64();
-            // 4x4 transposes inside the quad: afterwards a[4c + k] = gate k of (unit uk, chunk 4c + gj)
-#pragma unroll
-            for (int c = 0; c < NQ; ++c) {
-                float s0 = g0 ? a[4 * c + 0] : a[4 * c + 1];
-                float s1 = g0 ? a[4 * c + 2] : a[4 * c + 3];
-                float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
-                if (g0) { a[4 * c + 0] = r0; a[4 * c + 2] = r1; } else { a[4 * c + 1] = r0; a[4 * c + 3] = r1; }
-                s0 = g1 ? a[4 * c + 0] : a[4 * c + 2];
-                s1 = g1 ? a[4 * c + 1] : a[4 * c + 3];
-                r0 = __shfl_xor_sync(0xffffffffu, s0, 2);
-                r1 = __shfl_xor_sync(0xffffffffu, s1, 2);
-                if (g1) { a[4 * c + 0] = r0; a[4 * c + 1] = r1; } else { a[4 * c + 2] = r0; a[4 * c + 3] = r1; }
-            }
-            if (d) d[4] = clock64();
-            float hv[NQ];
-#pragma unroll
-            for (int c = 0; c < NQ; ++c) {
-                // outside the chunk (variable chunk sizes) the state is held at zero: a multiplicative mask, not a branch, so
-                // that the cells' transcendentals stay interleaved
-                const float alive = t < my_len[c] ? 1.0f : 0.0f;
-                const float cs = (a[4 * c + 1] * c_reg[c] + a[4 * c + 0] * a[4 * c + 2]) * alive;
-                c_reg[c] = cs;
-                hv[c] = a[4 * c + 3] * tanh_f(cs) * alive;
-            }
-            // Pair the units (uk, uk ^ 1): of the NQ / 2 chunk-quad pairs the even unit's lane stores the first half for both
-            // units and the odd unit's lane the second half, as 32-bit words (two adjacent units of one chunk row).
-            {
-                const bool odd = uk & 1;
-                const int ucol = qt * 8 + (uk & ~1);
-                constexpr int NP = NQ / 2;        // half2 pairs of chunk quads per lane: (hv[2i], hv[2i+1])
-#pragma unroll
-                for (int i = 0; i < NP / 2; ++i) {
-                    const __half2 first = __floats2half2_rn(hv[2 * i], hv[2 * i + 1]);
-                    const __half2 second = __floats2half2_rn(hv[2 * (NP / 2 + i)], hv[2 * (NP / 2 + i) + 1]);
-                    const uint32_t fu = *reinterpret_cast<const uint32_t*>(&first), su = *reinterpret_cast<const uint32_t*>(&second);
-                    const uint32_t got = __shfl_xor_sync(0xffffffffu, odd ? fu : su, 4);
-                    const uint32_t keep = odd ? su : fu;
-                    // keep = my h for quads (q0, q0+1), got = the partner unit's h for the same quads
-                    const uint32_t even_unit = odd ? got : keep, odd_unit = odd ? keep : got;
-                    const int q0 = 2 * (odd ? NP / 2 + i : i);
-                    const uint32_t w0 = (even_unit & 0xffffu) | (odd_unit << 16);          // chunk 4*q0 + gj
-                    const uint32_t w1 = (even_unit >> 16) | (odd_unit & 0xffff0000u);      // chunk 4*(q0+1) + gj
-                    *reinterpret_cast<uint32_t*>(stage + sw64_offset(4 * q0 + gj, ucol)) = w0;
-                    *reinterpret_cast<uint32_t*>(stage + sw64_offset(4 * (q0 + 1) + gj, ucol)) = w1;
-                }
-            }
-            if (d) d[5] = clock64();
-            tc::fence_proxy_async_smem();            // staged block -> visible to the bulk copy / TMA store
-            if (d) d[6] = clock64();
-            if (sender) tc::bulk_wait_group_read<0>();  // the store issued a step ago has read the other staging buffer
-            if (d) d[7] = clock64();
-            named_bar_sync(bar_id, 128);
-            if (d) d[8] = clock64();
-            if (sender) {
-                // all-gather over distributed shared memory: one bulk copy per destination CTA
-                if (s + 1 < steps) {
-#pragma unroll
-                    for (int rr = 0; rr < CL; ++rr) {
-                        tc::bulk_copy_smem_to_cluster(mapa_shared(dst_z[nbuf], (uint32_t)rr), tc::smem_u32(stage), (uint32_t)ZB,
-                                                      mapa_shared(dst_bar[nbuf], (uint32_t)rr));
-                    }
-                }
-                tc::tma_store_2d(&tma_y, stage, m * 32, t * p.N + nc0);
-                tc::bulk_commit_group();
-            }
-            if (d) d[9] = clock64();
         }
-        if (sender) tc::bulk_wait_group<0>();
+        // h_t has landed in every copy, and every thread is done with h_{t-1} and the gate buffer
+        if constexpr (CL > 1) cluster.sync();
+        else __syncthreads();
     }
-    tc::tc_fence_before();
-    __syncthreads();
-    // nobody leaves while a peer may still address this CTA's shared memory
-    cluster_arrive_release();
-    cluster_wait_acquire();
-    if (warp == 1) tc::tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
 }
 
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
 struct LstmLayerWeights {
-    __half* w = nullptr;   // resident path: [4C][2C] permuted rows, [W_ih | W_hh]
-    float* bias = nullptr; // [4C] permuted
-    // hoisted path (lstm_cluster_kernel): rows permuted as (tile, quarter, unit-in-quarter, gate)
-    __half* w_ih = nullptr;  // [4C][C]
+    __half* w_ih = nullptr;  // [4C][Cp] (K padded to a multiple of 64), PyTorch row order
     __half* w_hh = nullptr;  // [4C][C]
+    float* bias = nullptr;   // [4C] b_ih + b_hh
 };
 
 class LstmModel;
@@ -927,37 +495,27 @@ class LstmModel;
 class LstmPlan final : public ForwardPlan {
 public:
     void run(cudaStream_t stream, ProfileSink* prof) override;
-    int launches() const override { return 1 + 1 + num_layers * (hoisted ? 2 : 1) + num_linear; }
+    int launches() const override { return 1 + 1 + num_layers * 2 + num_linear; }
     std::string info() const override {
-        if (hoisted) return "lstm_rec.ctas=" + std::to_string(lstm_grid) + ";lstm_rec.chunks_per_cluster=" + std::to_string(rec_un);
-        return "lstm_layer.ctas=" + std::to_string(lstm_grid) + ";lstm_layer.groups=" + std::to_string(lstm_ng) +
-               ";lstm_layer.chunks_per_group=" + std::to_string(lstm_nbr);
+        return "lstm_rec.ctas=" + std::to_string(rec_ctas) + ";lstm_rec.chunks_per_cluster=" + std::to_string(rec_un);
     }
     void set_chunk_lengths(const int32_t* d_lens) override {
-        if (!hoisted) return;  // the mode exists for the cluster recurrence only
+        if (!variable) return;  // the mode exists for the models that run variable chunk sizes only
         conv12.lens = d_lens;
         for (auto& rp : rec_p) rp.lens = d_lens;
     }
 
     Conv12Params conv12{};
     dim3 conv12_grid;
-    bool conv12_tc = false;  // conv2 on tcgen05 (conv12_tc_kernel)
+    bool conv12_tc = false;  // conv2 on the tensor cores (conv12_tc_kernel)
     int conv12_tiles_per_chunk = 0, conv12_tc_grid = 0;
     GemmPlan conv3;
-    std::vector<CUtensorMap> lstm_x;
-    std::vector<LstmParams> lstm_p;
-    int lstm_grid = 0, lstm_nbr = 16, lstm_ng = 2;
-    size_t lstm_smem = 0;
-    void launch_lstm(int l, cudaStream_t stream) const;
-    // hoisted path
-    long long* dbg_timeline = nullptr;
     int debug_layers = -1;  // >= 0: stop after that many LSTM layers (B200_DEBUG_LSTM_LAYERS, read once at plan creation)
-    bool hoisted = false;
-    int rec_un = 32;       // chunks per cluster: 16 (one group of 16), 32 (two groups of 16) or 64 (two groups of 32)
+    bool variable = false;
+    int rec_un = 16;        // chunks per cluster (NB)
+    int rec_ctas = 0;
     std::vector<GemmPlan> gx_gemm;
-    std::vector<const __half*> rec_whh;
     std::vector<LstmRecParams> rec_p;
-    CUtensorMap rec_y_map; // seq as [T_out * Np][C], box 32 units x (chunks of a group): the TMA store of h_t
     void launch_rec(int l, cudaStream_t stream) const;
     GemmPlan linear1, linear2;
     int num_layers = 0, num_linear = 1;
@@ -973,7 +531,7 @@ public:
                                            size_t ws_bytes) override;
     bool variable_chunk_sizes() const override {
         // FLSTM models never run variable chunk sizes (api/runner_creation.cpp:28)
-        return hoisted() && desc.lstm_inner_dim == 0;
+        return large() && desc.lstm_inner_dim == 0;
     }
 
     b200_model_desc desc;
@@ -990,8 +548,10 @@ public:
 private:
     int pad3() const { return desc.convs[2].winlen / 2; }
     int t_pad(int T_in) const { return T_in + 2 * pad3() + 8; }
-    bool hoisted() const { return (size_t)4 * desc.lstm_size * 2 * desc.lstm_size * 2 > 150 * 1024; }
-    int n_pad(int N) const { return hoisted() ? (N + 31) / 32 * 32 : (N + 15) / 16 * 16; }
+    // lstm_size 96 keeps the reference's fixed-size contract (batch a multiple of 16, no variable chunk sizes); the larger
+    // sizes take batches in multiples of 32 and variable chunk sizes
+    bool large() const { return desc.lstm_size > 96; }
+    int n_pad(int N) const { return large() ? (N + 31) / 32 * 32 : (N + 15) / 16 * 16; }
 };
 
 LstmModel::LstmModel(const b200_model_desc& d, const b200_tensor* tensors, int n) : desc(d) {
@@ -1044,12 +604,12 @@ LstmModel::LstmModel(const b200_model_desc& d, const b200_tensor* tensors, int n
         w3 = upload_f16(w);
         b3 = upload_f32(std::vector<float>(tb.data, tb.data + C));
     }
-    // LSTM layers: permute gate rows into tiles of (i|f|g|o) x 32 units, concatenate [W_ih | W_hh]
+    // LSTM layers: W_ih (K padded for the GEMM), W_hh and the summed biases, gate rows in PyTorch order (i | f | g | o)
     for (int l = 0; l < d.lstm_layers; ++l) {
         const std::string pfx = std::to_string(d.num_convs + l + 1) + ".rnn.";
         // plain LSTM: the tensors as they are.  FLSTM (nn/FLSTMStack.cpp:18-25,108-124): gates = up_ih (dn_ih x_t) +
         // up_hh (dn_hh h_{t-1}) + bias, folded once into W = up x dn (double accumulation, rounded to fp32) so that the
-        // recurrence kernels -- and their weights-in-tensor-memory residency -- serve both model kinds.
+        // x-projection GEMM and the recurrence kernel serve both model kinds.
         struct View { const float* data; };
         std::vector<float> folded_ih, folded_hh;
         View wih{}, whh{}, bih{}, bhh{};
@@ -1085,34 +645,16 @@ LstmModel::LstmModel(const b200_model_desc& d, const b200_tensor* tensors, int n
             bih.data = find_tensor(tensors, n, pfx + "bias_ih_l0.tensor").data;
             bhh.data = find_tensor(tensors, n, pfx + "bias_hh_l0.tensor").data;
         }
-        std::vector<float> w((size_t)4 * C * 2 * C), b((size_t)4 * C);
-        for (int m = 0; m < C / 32; ++m)
-            for (int g = 0; g < 4; ++g)
-                for (int u = 0; u < 32; ++u) {
-                    const int dst = m * 128 + g * 32 + u;
-                    const int src = g * C + m * 32 + u;
-                    std::memcpy(&w[(size_t)dst * 2 * C], &wih.data[(size_t)src * C], sizeof(float) * C);
-                    std::memcpy(&w[(size_t)dst * 2 * C + C], &whh.data[(size_t)src * C], sizeof(float) * C);
-                    b[dst] = bih.data[src] + bhh.data[src];
-                }
-        LstmLayerWeights lw;
-        if ((size_t)4 * C * 2 * C * 2 <= 150 * 1024) {
-            lw.w = upload_f16(w);
-            lw.bias = upload_f32(b);
-        } else {
-            std::vector<float> wi((size_t)4 * C * C), wh((size_t)4 * C * C), b2((size_t)4 * C);
-            for (int m = 0; m < C / 32; ++m)
-                for (int r = 0; r < 128; ++r) {
-                    const int g = r & 3, unit = 32 * m + 8 * (r >> 5) + ((r & 31) >> 2);
-                    const int dst = m * 128 + r, src = g * C + unit;
-                    std::memcpy(&wi[(size_t)dst * C], &wih.data[(size_t)src * C], sizeof(float) * C);
-                    std::memcpy(&wh[(size_t)dst * C], &whh.data[(size_t)src * C], sizeof(float) * C);
-                    b2[dst] = bih.data[src] + bhh.data[src];
-                }
-            lw.w_ih = upload_f16(wi);
-            lw.w_hh = upload_f16(wh);
-            lw.bias = upload_f32(b2);
+        const int Cp = (C + 63) / 64 * 64;
+        std::vector<float> wi((size_t)4 * C * Cp, 0.0f), b((size_t)4 * C);
+        for (int r = 0; r < 4 * C; ++r) {
+            std::memcpy(&wi[(size_t)r * Cp], &wih.data[(size_t)r * C], sizeof(float) * C);
+            b[r] = bih.data[r] + bhh.data[r];
         }
+        LstmLayerWeights lw;
+        lw.w_ih = upload_f16(wi);
+        lw.w_hh = upload_f16(std::vector<float>(whh.data, whh.data + (size_t)4 * C * C));
+        lw.bias = upload_f32(b);
         layers.push_back(lw);
     }
     // linear(s)
@@ -1141,7 +683,6 @@ LstmModel::~LstmModel() {
     cudaFree(w3);
     cudaFree(b3);
     for (auto& l : layers) {
-        cudaFree(l.w);
         cudaFree(l.bias);
         cudaFree(l.w_ih);
         cudaFree(l.w_hh);
@@ -1156,7 +697,7 @@ size_t LstmModel::workspace_bytes(int N, int T_in) const {
     const size_t x2 = (size_t)N * t_pad(T_in) * 16 * 2 + 4096;
     const size_t seq = (size_t)(T_out + 1) * n_pad(N) * desc.lstm_size * 2 + 4096;
     const size_t mid = desc.out_features > 0 ? (size_t)T_out * n_pad(N) * desc.out_features * 2 + 4096 : 0;
-    const size_t gx = hoisted() ? (size_t)T_out * n_pad(N) * 4 * desc.lstm_size * 2 + 4096 : 0;
+    const size_t gx = (size_t)T_out * n_pad(N) * 4 * desc.lstm_size * 2 + 4096;
     return x2 + seq + mid + gx + 4096;  // + the tile counter of conv12_tc_kernel
 }
 
@@ -1167,7 +708,7 @@ std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half*
     const int Np = n_pad(N);
     if (Np != N) {
         // the reference's tensor-core LSTM has the same kind of constraint (multiples of 64, CudaCaller.h:60-63)
-        throw std::invalid_argument(hoisted() ? "batch_size must be a multiple of 32 for this LSTM size"
+        throw std::invalid_argument(large() ? "batch_size must be a multiple of 32 for this LSTM size"
                                               : "batch_size must be a multiple of 16 for LSTM models");
     }
     auto plan = std::make_unique<LstmPlan>();
@@ -1184,7 +725,7 @@ std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half*
     __half* x2 = reinterpret_cast<__half*>(take((size_t)N * Tp * 16 * 2));
     __half* seq = reinterpret_cast<__half*>(take((size_t)(T_out + 1) * Np * C * 2));
     __half* mid = desc.out_features > 0 ? reinterpret_cast<__half*>(take((size_t)T_out * Np * desc.out_features * 2)) : nullptr;
-    __half* gxbuf = hoisted() ? reinterpret_cast<__half*>(take((size_t)T_out * Np * 4 * C * 2)) : nullptr;
+    __half* gxbuf = reinterpret_cast<__half*>(take((size_t)T_out * Np * 4 * C * 2));
     int* tile_counter = reinterpret_cast<int*>(take(256));
 
     // conv1 + conv2
@@ -1192,6 +733,7 @@ std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half*
                                 desc.convs[1].winlen, desc.convs[0].activation, desc.convs[1].activation, nullptr, tile_counter};
     plan->conv12_grid = dim3((T_in + CONV_TT - 1) / CONV_TT, N, 1);
     // the v5 shape runs conv2 on the tensor cores (conv12_tc_kernel); anything else keeps the FMA-pipe kernel
+    // (B200_CONV12_FMA=1 forces it: the tests compare the two)
     plan->conv12_tc = desc.convs[0].size == 16 && desc.convs[1].winlen == 5 && !std::getenv("B200_CONV12_FMA");
     plan->conv12_tiles_per_chunk = (T_in + C12_TILE - 1) / C12_TILE;
     {
@@ -1220,122 +762,61 @@ std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half*
         g.out_s1 = (int64_t)Np * C;  // t
         plan->conv3 = make_gemm_plan(g);
     }
-    // LSTM layers
-    if (hoisted()) {
+    // LSTM layers: x-projection GEMM + cluster recurrence
+    {
         plan->num_layers = desc.lstm_layers;
-        plan->hoisted = true;
-        if (C != 192 && C != 384) throw Unsupported("hoisted LSTM path is instantiated for lstm_size 192 and 384");
-        // Weights-stationary cluster kernel (6 CTAs per cluster).  Chunks per cluster: a step costs about the same for 16, 32 or
-        // 64 chunks, so fewer and fatter clusters do the same work in fewer SM-cycles at a higher latency per launch.  With R
-        // runners in flight the recurrence takes ~1/R of the SMs (64 chunks per cluster: 8 clusters = 48 SMs at batch 512,
-        // three batches' recurrences side by side); a lone runner spreads out (32 per cluster = 96 SMs, 16 for small batches).
-        const int hint = num_runners_hint < 1 ? 1 : num_runners_hint;
-        int un = Np > 256 ? 32 : 16;
-        if (hint >= 2 && Np % 64 == 0 && (Np / 32) * 6 > 148 / hint) un = 64;
+        plan->variable = variable_chunk_sizes();
+        const int CL = rec_cluster(C);
+        // Chunks per cluster: 32 for large batches, 16 below.  64 chunks (B200_CLUSTER_CHUNKS=64) spill registers next to
+        // the register-resident W_hh of lstm_size 384 and were no faster: hac batch 512, 4 runners, 77.6 vs 77.7 Msamples/s
+        // for 64 vs 32 (two alternating runs each, NVIDIA H100 80GB HBM3 at 700 W).  lstm_size 96 (one CTA per cluster)
+        // stays at 16.
+        int un = 16;
+        if (CL > 1 && Np > 256) un = 32;
         if (const char* e = std::getenv("B200_CLUSTER_CHUNKS")) {   // tuning / A-B override
             const int v = std::atoi(e);
             if ((v == 16 || v == 32 || v == 64) && Np % v == 0) un = v;
             else throw std::invalid_argument("B200_CLUSTER_CHUNKS must be 16, 32 or 64 and divide the padded batch");
         }
+        // one CTA of 8 x 96 threads cannot hold the accumulators of 64 chunks without spilling
+        if (CL == 1 && un > 32) un = 32;
         while (Np % un != 0) un /= 2;
         plan->rec_un = un;
-        plan->rec_y_map = make_tmap_2d(seq, (uint64_t)C, (uint64_t)T_out * Np, (uint64_t)C * 2, 32, un == 64 ? 32 : 16);
-        const int GB = 32;  // chunk block of the gx layout (n_pad = 32 on this path)
-        // With three or more batches in flight the x-projection GEMMs keep off 32 SMs, so that another batch's recurrence
-        // (48 SMs, several milliseconds of latency chain) can start beside them instead of queueing behind a GEMM that owns every SM
-        // (measured at batch 512, 4 runners: 26.4 -> 24.0 ms per step in battery 13, whose files were lost; after the tile-order change
-        // caps of 100-148 are within the run-to-run spread, profiles/r02_b26_bench_hac_cap*).
-        const int gemm_cap = hint >= 3 ? 116 : 0;
-        plan->lstm_grid = (Np / un) * 6;
+        plan->rec_ctas = (Np / un) * CL;
+        // With three or more batches in flight the x-projection GEMMs keep off some SMs, so that another batch's recurrence
+        // (several milliseconds of latency chain) can start beside them instead of queueing behind a GEMM that owns every SM.
+        const int hint = num_runners_hint < 1 ? 1 : num_runners_hint;
+        const int gemm_cap = hint >= 3 ? kNumSMs - 32 : 0;
+        const int Cp = (C + 63) / 64 * 64;
         for (int l = 0; l < desc.lstm_layers; ++l) {
             GemmDesc g{};
-            g.a = layers[l].w_ih;  // gate rows are the M dimension, (t, chunk) the N dimension
+            g.a = seq;   // rows (t, chunk), K = the layer input
             g.batches = 1;
-            g.rows_per_batch = 4 * C;
+            g.rows_per_batch = T_out * Np;
             g.a_row_stride = C;
-            g.a_batch_stride = (int64_t)4 * C * C;
-            g.w = seq;
-            g.N = T_out * Np;
-            g.K = C;
+            g.a_batch_stride = (int64_t)T_out * Np * C;
+            g.a_inner = C;
+            g.w = layers[l].w_ih;
+            g.N = 4 * C;
+            g.K = Cp;
             g.bias = layers[l].bias;
-            g.bias_per_row = 1;
             g.act = GEMM_ACT_NONE;
             g.out = gxbuf;
             g.out_m1 = 1;
-            g.out_s0 = GB;
-            g.out_col_m1 = GB;
-            g.out_col_s0 = (int64_t)4 * C * GB;
+            g.out_s0 = 4 * C;
             g.max_ctas = gemm_cap;
             plan->gx_gemm.push_back(make_gemm_plan(g));
-            plan->rec_whh.push_back(layers[l].w_hh);
             LstmRecParams rp{};
             rp.seq = seq;
             rp.gx = gxbuf;
+            rp.w_hh = layers[l].w_hh;
             rp.T = T_out;
             rp.N = Np;
-            rp.reverse = (l % 2 == 0) ? 1 : 0;
+            rp.reverse = (l % 2 == 0) ? 1 : 0;  // reverse_first = true (CRFModel.cpp:40, LSTMStack.cpp:31-41)
             rp.lens = nullptr;
             rp.stride = desc.stride;
-            rp.dbg = nullptr;
-            if (l == 0 && getenv("B200_DEBUG_LSTM_TIMELINE")) {
-                B200_CUDA(cudaMalloc(&rp.dbg, 128 * sizeof(long long)));
-                B200_CUDA(cudaMemset(rp.dbg, 0, 128 * sizeof(long long)));
-                plan->dbg_timeline = rp.dbg;
-            }
             plan->rec_p.push_back(rp);
         }
-    } else {
-        plan->num_layers = desc.lstm_layers;
-        if (C != 96) throw Unsupported("the single-CTA LSTM kernel is instantiated for lstm_size 96");
-        // Grid shape.  A step costs a dependent chain of ~1000-2200 cycles whether a group holds 2 or 8 chunks, so SM-time per
-        // chunk falls with chunks per CTA while the latency of one launch rises.  With R runners (batches) in flight the
-        // recurrence is therefore sized for ~1/R of the SMs, two groups per CTA, and runs side by side with the other
-        // batches' recurrences and decodes (measured at batch 512, profiles/r02_b10_*, r02_b11_*: 4 runners x 32 CTAs x
-        // 2 x 8 chunks 5.76 ms/step; 2 runners x 64 CTAs x 2 x 4 chunks 7.27; 2 runners x 128 CTAs x 1 x 4 chunks 8.0-8.9).  A lone
-        // runner has nothing to overlap with: one group of 4 chunks on every SM is fastest (0.98 vs 1.17 ms per layer).
-        const int hint = num_runners_hint < 1 ? 1 : num_runners_hint;
-        int ng = hint == 1 ? 1 : 2, nbr = 16;
-        if (const char* e = std::getenv("B200_LSTM_GROUPS")) ng = std::atoi(e) == 1 ? 1 : 2;   // A/B comparisons
-        if (Np % (2 * ng) != 0) ng = 1;
-        const int target = 148 / hint > 0 ? 148 / hint : 1;
-        const int min_nbr = ng == 1 ? 4 : 2;
-        for (int v = min_nbr; v <= 16; v *= 2) {
-            if (Np % (v * ng) == 0 && (Np / (v * ng) <= target || v == 16)) {
-                nbr = v;
-                break;
-            }
-        }
-        if (Np % (nbr * ng) != 0) ng = 1;   // Np is a multiple of 16
-        // tuning override: with several runners in flight, fatter CTAs (fewer SMs per kernel) let the recurrences of
-        // different batches run side by side instead of queueing for the same SMs
-        if (const char* e = std::getenv("B200_LSTM_CHUNKS_PER_CTA")) {
-            const int v = std::atoi(e);
-            if ((v == 2 || v == 4 || v == 8 || v == 16) && Np % (v * ng) == 0) nbr = v;
-            else throw std::invalid_argument("B200_LSTM_CHUNKS_PER_CTA must be 2, 4, 8 or 16 and divide the padded batch");
-        }
-        plan->lstm_nbr = nbr;
-        plan->lstm_ng = ng;
-        plan->lstm_grid = Np / (nbr * ng);
-        plan->lstm_smem = ng == 2 ? LstmCfg<96, 2>::smem_bytes(nbr) : LstmCfg<96, 1>::smem_bytes(nbr);
-        for (int l = 0; l < desc.lstm_layers; ++l) {
-            plan->lstm_x.push_back(make_tmap_2d(seq, (uint64_t)C, (uint64_t)T_out * Np, (uint64_t)C * 2, KBLK, nbr));
-            LstmParams lp{};
-            lp.seq = seq;
-            lp.bias = layers[l].bias;
-            lp.w = layers[l].w;
-            lp.T = T_out;
-            lp.N = Np;
-            lp.C = C;
-            lp.reverse = (l % 2 == 0) ? 1 : 0;  // reverse_first = true (CRFModel.cpp:40, LSTMStack.cpp:31-41)
-            lp.dbg = nullptr;
-            if (l == 0 && getenv("B200_DEBUG_LSTM_TIMELINE")) {
-                B200_CUDA(cudaMalloc(&lp.dbg, 64 * sizeof(long long)));
-                B200_CUDA(cudaMemset(lp.dbg, 0, 64 * sizeof(long long)));
-                plan->dbg_timeline = lp.dbg;
-            }
-            plan->lstm_p.push_back(lp);
-        }
-        if (plan->lstm_smem > 227 * 1024) throw Unsupported("LSTM shared-memory plan does not fit");
     }
     // linear CRF (+ optional decomposition); rows g = t * Np + n  ->  scores[n][t][:]
     {
@@ -1386,18 +867,12 @@ std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half*
     return plan;
 }
 
-template <int C, int NBR, int NG>
-static void launch_lstm_t(const LstmPlan& pl, int l, cudaStream_t stream) {
-    ensure_dynamic_smem(lstm_layer_kernel<C, NBR, NG>, (int)LstmCfg<C, NG>::smem_bytes(NBR));
-    lstm_layer_kernel<C, NBR, NG><<<pl.lstm_grid, LstmCfg<C, NG>::THREADS, pl.lstm_smem, stream>>>(pl.lstm_x[l], pl.lstm_p[l]);
-}
-
-template <int C, int CL, int NG, int GN>
-static void launch_cluster_t(const LstmPlan& pl, int l, cudaStream_t stream) {
-    using Cfg = ClusterCfg<C, CL, NG, GN>;
-    ensure_dynamic_smem(lstm_cluster_kernel<C, CL, NG, GN>, (int)Cfg::SMEM);
+template <int C, int CL, int NB>
+static void launch_rec_t(const LstmRecParams& rp, int ctas, cudaStream_t stream) {
+    using Cfg = RecCfg<C, CL, NB>;
+    ensure_dynamic_smem(lstm_rec_kernel<C, CL, NB>, (int)Cfg::SMEM);
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)pl.lstm_grid, 1, 1);
+    cfg.gridDim = dim3((unsigned)ctas, 1, 1);
     cfg.blockDim = dim3(Cfg::THREADS, 1, 1);
     cfg.dynamicSmemBytes = Cfg::SMEM;
     cfg.stream = stream;
@@ -1408,48 +883,28 @@ static void launch_cluster_t(const LstmPlan& pl, int l, cudaStream_t stream) {
     at[0].val.clusterDim.z = 1;
     cfg.attrs = at;
     cfg.numAttrs = 1;
-    B200_CUDA(cudaLaunchKernelEx(&cfg, lstm_cluster_kernel<C, CL, NG, GN>, pl.rec_y_map, pl.rec_whh[l], pl.rec_p[l]));
+    B200_CUDA(cudaLaunchKernelEx(&cfg, lstm_rec_kernel<C, CL, NB>, rp));
 }
 
 template <int C>
-static void launch_cluster_c(const LstmPlan& pl, int l, cudaStream_t stream) {
-    switch (pl.rec_un) {
-        case 64: launch_cluster_t<C, 6, 2, 32>(pl, l, stream); break;
-        case 32: launch_cluster_t<C, 6, 2, 16>(pl, l, stream); break;
-        default: launch_cluster_t<C, 6, 1, 16>(pl, l, stream); break;
+static void launch_rec_c(const LstmRecParams& rp, int un, int ctas, cudaStream_t stream) {
+    constexpr int CL = rec_cluster(C);
+    switch (un) {
+        case 64:
+            if constexpr (CL > 1) launch_rec_t<C, CL, 64>(rp, ctas, stream);
+            else throw std::logic_error("lstm recurrence: 64 chunks per single-CTA cluster");
+            break;
+        case 32: launch_rec_t<C, CL, 32>(rp, ctas, stream); break;
+        default: launch_rec_t<C, CL, 16>(rp, ctas, stream); break;
     }
 }
 
 void LstmPlan::launch_rec(int l, cudaStream_t stream) const {
-    const int C = model->desc.lstm_size;
-    if (C == 384) launch_cluster_c<384>(*this, l, stream);
-    else if (C == 192) launch_cluster_c<192>(*this, l, stream);
-    else throw Unsupported("no cluster LSTM kernel instantiation for this lstm_size");
-}
-
-template <int C>
-static void launch_lstm_c(const LstmPlan& pl, int l, cudaStream_t stream) {
-    if (pl.lstm_ng == 2) {
-        switch (pl.lstm_nbr) {
-            case 2: launch_lstm_t<C, 2, 2>(pl, l, stream); break;
-            case 4: launch_lstm_t<C, 4, 2>(pl, l, stream); break;
-            case 8: launch_lstm_t<C, 8, 2>(pl, l, stream); break;
-            default: launch_lstm_t<C, 16, 2>(pl, l, stream); break;
-        }
-    } else {
-        switch (pl.lstm_nbr) {
-            case 2: launch_lstm_t<C, 2, 1>(pl, l, stream); break;
-            case 4: launch_lstm_t<C, 4, 1>(pl, l, stream); break;
-            case 8: launch_lstm_t<C, 8, 1>(pl, l, stream); break;
-            default: launch_lstm_t<C, 16, 1>(pl, l, stream); break;
-        }
-    }
-}
-
-void LstmPlan::launch_lstm(int l, cudaStream_t stream) const {
-    switch (lstm_p[l].C) {
-        case 96: launch_lstm_c<96>(*this, l, stream); break;
-        default: throw Unsupported("no LSTM kernel instantiation for this lstm_size");
+    switch (model->desc.lstm_size) {
+        case 96: launch_rec_c<96>(rec_p[l], rec_un, rec_ctas, stream); break;
+        case 192: launch_rec_c<192>(rec_p[l], rec_un, rec_ctas, stream); break;
+        case 384: launch_rec_c<384>(rec_p[l], rec_un, rec_ctas, stream); break;
+        default: throw Unsupported("no LSTM recurrence instantiation for this lstm_size");
     }
 }
 
@@ -1472,42 +927,14 @@ void LstmPlan::run(cudaStream_t stream, ProfileSink* prof) {
         const int nl = debug_layers >= 0 && debug_layers < num_layers ? debug_layers : num_layers;
         for (int l = 0; l < nl; ++l) {
             NvtxRange r("lstm_layer");
-            if (hoisted) {
-                run_gemm(gx_gemm[l], stream);
-                if (prof) prof->mark("lstm_gx_gemm", stream);
-                launch_rec(l, stream);
-                if (prof) prof->mark("lstm_rec", stream);
-            } else {
-                launch_lstm(l, stream);
-                if (prof) prof->mark("lstm_layer", stream);
-            }
+            run_gemm(gx_gemm[l], stream);
+            if (prof) prof->mark("lstm_gx_gemm", stream);
+            launch_rec(l, stream);
+            if (prof) prof->mark("lstm_rec", stream);
         }
         if (nl < num_layers) {  // debug: stop after nl layers (tools/debug_forward.py reads the sequence buffer)
             B200_CUDA(cudaGetLastError());
             return;
-        }
-    }
-    if (dbg_timeline) {
-        long long h[128];
-        B200_CUDA(cudaStreamSynchronize(stream));
-        B200_CUDA(cudaMemcpy(h, dbg_timeline, hoisted ? sizeof(h) : 64 * sizeof(long long), cudaMemcpyDeviceToHost));
-        for (int s = 0; s < 4; ++s) {
-            if (hoisted) {
-                const long long* e = h + s * 32;
-                const long long t0 = e[0];
-                fprintf(stderr, "[cluster timeline step %d] mma g0: wait %lld..%lld issued %lld | g1: wait %lld..%lld issued %lld | epi(g0,t0): "
-                                "wait_acc %lld..%lld ld %lld act %lld transpose %lld cells+stage %lld fence %lld wait_read %lld bar %lld sent %lld | "
-                                "period %lld\n",
-                        64 + s, e[0] - t0, e[1] - t0, e[2] - t0, e[4] - t0, e[5] - t0, e[6] - t0, e[8] - t0, e[9] - t0, e[10] - t0, e[11] - t0,
-                        e[12] - t0, e[13] - t0, e[14] - t0, e[15] - t0, e[16] - t0, e[17] - t0, s > 0 ? e[0] - (e - 32)[0] : 0LL);
-            } else {
-                const long long* e = h + s * 16;
-                const long long t0 = e[0];
-                fprintf(stderr, "[lstm timeline step %d] mma: wait_h 0..%lld issued %lld | epi: wait_acc %lld..%lld ld %lld act %lld "
-                                "transpose/bar %lld cells %lld fence %lld arrive %lld store %lld | period %lld\n",
-                        64 + s, e[1] - t0, e[2] - t0, e[4] - t0, e[5] - t0, e[6] - t0, e[7] - t0, e[8] - t0, e[9] - t0, e[10] - t0, e[11] - t0,
-                        e[12] - t0, s > 0 ? e[0] - (e - 16)[0] : 0LL);
-            }
         }
     }
     NvtxRange r("linear");

@@ -1,5 +1,5 @@
-// sm_100a building blocks: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM) wrappers.
-// Hand-written inline PTX; descriptor bit layouts follow the PTX ISA "tcgen05 matrix descriptors".
+// sm_90a building blocks: mbarrier, TMA (cp.async.bulk.tensor), wgmma and mma.sync wrappers.
+// Hand-written inline PTX; descriptor bit layouts follow the PTX ISA "matrix descriptor format" of wgmma.
 #pragma once
 
 #include <cuda.h>
@@ -45,6 +45,15 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
             printf("b200: mbarrier wait timeout (block %d thread %d)\n", (int)blockIdx.x, (int)threadIdx.x);
             __trap();
         }
+    }
+}
+
+// The same without the printf: a function call anywhere in a kernel that issues wgmma makes ptxas serialise the wgmma
+// instructions (C7510).
+__device__ __forceinline__ void mbar_wait_silent(uint64_t* bar, uint32_t parity) {
+    uint32_t spins = 0;
+    while (!mbar_try_wait(bar, parity)) {
+        if (++spins > (1u << 26)) __trap();
     }
 }
 
@@ -98,123 +107,64 @@ __device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUte
             ::"r"(smem_u32(smem_dst)), "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
             : "memory");
 }
-// generic-proxy writes (st.shared) -> visible to the async proxy (UMMA / TMA reads of smem)
+// generic-proxy writes (st.shared) -> visible to the async proxy (wgmma / TMA reads of smem)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---------------------------------------------------------------- TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_holder, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread = TMEM lane)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-            "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-            : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-              "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-              "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-              "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-            : "r"(taddr)
-            : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-            "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-            : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-              "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-            : "r"(taddr)
-            : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x8(uint32_t taddr, uint32_t* r) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x4(uint32_t taddr, uint32_t* r) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-                 : "r"(taddr)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x2(uint32_t taddr, uint32_t* r) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0,%1}, [%2];" : "=r"(r[0]), "=r"(r[1]) : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---------------------------------------------------------------- UMMA descriptors
-// Shared-memory matrix descriptor, K-major operand stored as rows of 128 B (64 fp16) with the
-// 128-byte swizzle TMA produces (CU_TENSOR_MAP_SWIZZLE_128B): 8-row groups 1024 B apart.
-//   [0,14)  start address >> 4      [16,30) leading byte offset >> 4 (ignored for swizzled K-major; 1)
-//   [32,46) stride byte offset >> 4 (1024 B between 8-row groups)   [46,48) version = 1 (sm_100)
-//   [61,64) layout type: 2 = SWIZZLE_128B
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// ---------------------------------------------------------------- warpgroup MMA (wgmma)
+// Shared-memory matrix descriptor, K-major operand stored as rows of 128 B (64 fp16) with the 128-byte swizzle TMA produces
+// (CU_TENSOR_MAP_SWIZZLE_128B): 8-row groups 1024 B apart.
+//   [0,14)  start address >> 4      [16,30) leading byte offset >> 4 (unused for swizzled K-major; 1)
+//   [32,46) stride byte offset >> 4 (1024 B between 8-row groups)   [62,64) layout type: 1 = SWIZZLE_128B
+// Advancing 16 fp16 (32 B) along K inside the swizzle row is +2 in the address field.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3ffffu) >> 4);
     d |= (uint64_t)1 << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// Instruction descriptor for kind::f16: fp16 A/B (K-major), fp32 accumulate, M x N tile.
-//   [4,6) D format 1=f32   [7,10) A format 0=f16   [10,13) B format 0=f16   [15] A major 0=K   [16] B major 0=K
-//   [17,23) N>>3   [24,29) M>>4
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, bool accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x 32] (+)= A[64 x 16] B[16 x 32]^T, both K-major in shared memory, fp16 in, fp32 accumulate.  Thread t of the
+// warpgroup holds rows 16 (t / 32) + (t % 32) / 4 (+ 8) and columns 8 j + 2 (t % 4) (+ 1): d[4 j + {0, 1}] row r,
+// d[4 j + {2, 3}] row r + 8.
+__device__ __forceinline__ void wgmma_m64n32k16(float* d, uint64_t adesc, uint64_t bdesc, bool accumulate) {
     asm volatile(
             "{\n\t.reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-            ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"((uint32_t)accumulate)
+            "setp.ne.b32 p, %18, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+            "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+              "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(adesc), "l"(bdesc), "r"((uint32_t)accumulate)
             : "memory");
 }
-// A operand from tensor memory (lane = row of the 128-row tile, one 32-bit column = two fp16 along K), B from smem
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, bool accumulate) {
-    asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-            ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"((uint32_t)accumulate)
-            : "memory");
+
+// ---------------------------------------------------------------- warp MMA (mma.sync) and ldmatrix
+// The latency-bound kernels (recurrence, conv2, attention) work on warp-sized tiles with the operands in registers.
+// m16n8k16: a[4] = A rows (l / 4, + 8) x k pairs (2 (l % 4), + 8); b[2] = B k pairs (2 (l % 4), + 8) x column l / 4;
+// c[4] = rows (l / 4, + 8) x columns 2 (l % 4) + {0, 1}.
+__device__ __forceinline__ void mma_f16_16816(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-// registers -> TMEM: thread = lane, 32 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t* r) {
-    asm volatile(
-            "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-            "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-            "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-            ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-              "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-              "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-              "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-            : "memory");
+__device__ __forceinline__ void ldmatrix_x4(uint32_t* r, uint32_t smem_addr) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+                 : "r"(smem_addr));
 }
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t* r) {
-    asm volatile(
-            "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-            "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-            ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-              "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-            : "memory");
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t* r, uint32_t smem_addr) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+                 : "r"(smem_addr));
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// All previously issued MMAs of this thread arrive on `bar` when complete (implies fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
+__device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
+    const __half2 h = __floats2half2_rn(lo, hi);
+    return *reinterpret_cast<const uint32_t*>(&h);
 }
 
 __device__ __forceinline__ bool elect_one() {

@@ -1,4 +1,4 @@
-// Conv -> Transformer encoder -> upsample -> scaled CRF linear forward (sup models) for sm_100a.
+// Conv -> Transformer encoder -> upsample -> scaled CRF linear forward (sup models) for sm_90a.
 //
 // Replaces the CUDA path of dorado/basecall/model/TxModel.cpp:20-41 and dorado/nn/TxModules.cpp:
 //   conv stack (torch conv1d on the reference's CUDA path)   ConvStack.cpp:146-163    -> conv1 kernel + gemm.cu
@@ -7,11 +7,11 @@
 //   koi_mm_swiglu                                            TxModules.cpp:683        -> gemm.cu (SwiGLU epilogue)
 //   LinearUpsample, LinearScaledCRF                          LinearUpsample.cpp:17-23, TxModules.cpp:1010-1016 -> gemm.cu
 // Semantics follow the CPU modules: TxEncoderImpl::forward (TxModules.cpp:859-906), MultiHeadAttentionImpl
-// (:346-426, true window -win_upper <= j - i <= win_lower, see DESIGN.md on the CPU split quirk), RotaryEmbedding
+// (:346-426, true window -win_upper <= j - i <= win_lower, see oracle/nn_oracle.py on the CPU split quirk), RotaryEmbedding
 // (:220-250, half-split rotation), GatedMLP (:170-176), RMSNorm (RMSNorm.cpp:14-18).
 //
 // Activations are NTC fp16.  Every conv after the first is a strided GEMM over the zero-padded NTC buffer of
-// the previous layer (row stride = stride * C_in), all projections are tcgen05 GEMMs; the residual stream is
+// the previous layer (row stride = stride * C_in), all projections are wgmma GEMMs; the residual stream is
 // x <- RMSNorm(sublayer(x) + alpha * x) with the "+ alpha * x" fused into the GEMM epilogue.
 #include "engine.h"
 #include "gemm.h"
@@ -111,29 +111,23 @@ __global__ void __launch_bounds__(256) rmsnorm512_kernel(const __half* __restric
 constexpr int ATT_D = 64;   // head dimension
 
 // ------------------------------------------------------------------------------------------------
-// Sliding-window attention on the 5th-generation tensor cores (successor of koi_masked_attention, TxModules.cpp:648;
-// window semantics TxModules.cpp:310-317: keys j with -win_upper <= j - i <= win_lower).
+// Sliding-window attention on the tensor cores (successor of koi_masked_attention, TxModules.cpp:648; window semantics
+// TxModules.cpp:310-317: keys j with -win_upper <= j - i <= win_lower).
 // qkv: [N*T][3][H][64] fp16 (output of the Wqkv GEMM, q and k already rotated); out: [N*T][H*64] fp16.
 // One CTA = 128 queries of one (chunk, head); the keys they can see lie in at most three aligned blocks of 128 keys (the
-// kernel requires win_upper + win_lower + 128 <= 3 * 128), walked flash-style:
-//     S_b = Q K_b^T         tcgen05.mma, 128 x 128 x 64, Q and K_b in shared memory (TMA, 128-byte swizzle), S_b in TMEM
-//     P_b = exp2(S_b' - m)  one thread per query row (TMEM lane): tcgen05.ld S, running max / sum, P packed to fp16 and
-//                           written back into TENSOR MEMORY with tcgen05.st -- over the S columns it has consumed
-//     O_b = P_b V_b         tcgen05.mma with A = P read from TMEM and B = V_b as it lies in memory ([key][d], i.e. the
-//                           MN-major form of the B operand -- no transposed copy of V is ever made)
-//     O   = O * alpha + O_b in registers (64 fp32 per row), so the accumulator in TMEM is never rescaled in place
-// Tensor memory holds two 128-column buffers; buffer b & 1 carries S_b, then P_b in its columns 0-63 and O_b in its columns
-// 64-127.  That lets the issuer run ahead: S_1 is computed while the rows are still in the softmax of block 0, P_0 V_0 runs
-// under the softmax of block 1, and the rows fold O_b in one block late -- the dependent chain S -> softmax -> PV of a block
-// is off the critical path except at the ends.  All three K/V blocks are loaded up front (V in three buffers, K_2 reuses K_0's
-// buffer once S_0 has completed).
-// Warp roles: warp 0 TMA producer, warp 1 MMA issuer, warps 2-5 the 128 softmax rows.  TMEM 256 columns, shared memory 97 KB:
-// two CTAs share an SM.
+// kernel requires win_upper + win_lower + 128 <= 3 * 128).  One thread loads Q and every K / V block up front by TMA
+// (128-byte swizzle); each of the eight warps then owns 16 query rows and walks the blocks flash-style on mma.sync:
+//     S_b = Q K_b^T          16 x 128 per warp, fp32 in registers (Q and K_b fragments by ldmatrix)
+//     P_b = exp2(S_b' - m)   running max / sum per row (the four lanes of a quad share a row), P rounded to fp16 and
+//                            re-used in registers as the A fragments of the next product
+//     O = O * alpha + P_b V_b  V_b as it lies in memory ([key][d]) through ldmatrix.trans -- no transposed copy of V
+// Shared memory 113 KB: two CTAs share an SM.
 // ------------------------------------------------------------------------------------------------
 constexpr int AT_BQ = 128, AT_BK = 128;
 constexpr int AT_TILE = 128 * 64 * 2;   // one [128 x 64] fp16 tile
 constexpr int AT_MAXBLK = 3;
-constexpr int AT_SMEM = 1024 + (1 + 2 + AT_MAXBLK) * AT_TILE + 256;
+constexpr int AT_THREADS = 256;
+constexpr int AT_SMEM = 1024 + (1 + 2 * AT_MAXBLK) * AT_TILE + 64;
 
 struct AttnTcParams {
     __half* out;   // [N*T][H*64]
@@ -141,33 +135,15 @@ struct AttnTcParams {
     int win_upper, win_lower;
 };
 
-__device__ __forceinline__ uint64_t umma_desc_sw128_mn(uint32_t smem_addr) {
-    // B operand stored [K rows][64 N-elements = 128 B]: MN-major, 128-byte swizzle, 8-row (K) groups 1024 B apart.  The tile
-    // is one swizzle atom wide in N, so only the K-direction stride matters; both offset fields carry it.
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3ffffu) >> 4);
-    d |= (uint64_t)(1024 >> 4) << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-
-__global__ void __launch_bounds__(192, 2) tx_attention_tc_kernel(const __grid_constant__ CUtensorMap tma_qkv, const AttnTcParams p) {
+__global__ void __launch_bounds__(AT_THREADS, 2) tx_attention_tc_kernel(const __grid_constant__ CUtensorMap tma_qkv, const AttnTcParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* q_s = smem;                       // [128 q][64 d]
-    uint8_t* k_s = q_s + AT_TILE;              // [2][128 keys][64 d]   block b in buffer b & 1
-    uint8_t* v_s = k_s + 2 * AT_TILE;          // [3][128 keys][64 d]   block b in buffer b
+    uint8_t* q_s = smem;                          // [128 q][64 d]
+    uint8_t* k_s = q_s + AT_TILE;                 // [3][128 keys][64 d]
+    uint8_t* v_s = k_s + AT_MAXBLK * AT_TILE;     // [3][128 keys][64 d]
     uint64_t* bars = reinterpret_cast<uint64_t*>(v_s + AT_MAXBLK * AT_TILE);
-    uint64_t* q_full = bars;          // TMA -> MMA
-    uint64_t* kv_full = bars + 1;     // [3] TMA -> MMA
-    uint64_t* k_free = bars + 4;      // S_0 has completed: K buffer 0 may take block 2
-    uint64_t* s_full = bars + 5;      // [2] MMA -> softmax
-    uint64_t* p_ready = bars + 7;     // [2] softmax wrote P -> MMA (4 warp arrivals)
-    uint64_t* o_full = bars + 9;      // [2] MMA -> softmax
-    uint64_t* buf_free = bars + 11;   // [2] softmax has read O_b: the TMEM buffer may take S of block b + 2 (4 warp arrivals)
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 13);
+    uint64_t* q_full = bars;          // TMA -> warps
+    uint64_t* kv_full = bars + 1;     // [3]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int qt = blockIdx.x, h = blockIdx.y, n = blockIdx.z;
@@ -179,206 +155,135 @@ __global__ void __launch_bounds__(192, 2) tx_attention_tc_kernel(const __grid_co
     const int kb_max = (p.T - 1) / AT_BK;
     if (kb_last > kb_max) kb_last = kb_max;
     const int nblk = kb_last - kb_first + 1;     // 1..3 (checked on the host)
+    const int row0 = n * p.T;   // first token row of this chunk in the [N*T][1536] view
 
     if (threadIdx.x == 0) {
         tc::mbar_init(q_full, 1);
         for (int i = 0; i < AT_MAXBLK; ++i) tc::mbar_init(&kv_full[i], 1);
-        tc::mbar_init(k_free, 1);
-        for (int i = 0; i < 2; ++i) {
-            tc::mbar_init(&s_full[i], 1);
-            tc::mbar_init(&p_ready[i], 4);
-            tc::mbar_init(&o_full[i], 1);
-            tc::mbar_init(&buf_free[i], 4);
-        }
         tc::fence_barrier_init();
         tc::prefetch_tmap(&tma_qkv);
+        tc::mbar_arrive_expect_tx(q_full, AT_TILE);
+        tc::tma_load_2d(q_s, &tma_qkv, q_full, h * ATT_D, row0 + q0);
+        for (int b = 0; b < nblk; ++b) {
+            tc::mbar_arrive_expect_tx(&kv_full[b], 2 * AT_TILE);
+            const int krow = row0 + (kb_first + b) * AT_BK;
+            tc::tma_load_2d(k_s + b * AT_TILE, &tma_qkv, &kv_full[b], (p.H + h) * ATT_D, krow);
+            tc::tma_load_2d(v_s + b * AT_TILE, &tma_qkv, &kv_full[b], (2 * p.H + h) * ATT_D, krow);
+        }
     }
-    if (warp == 1) tc::tmem_alloc(tmem_holder, 256);
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_base = *tmem_holder;
-    const int row0 = n * p.T;   // first token row of this chunk in the [N*T][1536] view
 
-    if (warp == 0) {
-        // ---------------- TMA producer: everything up front ----------------
-        if (tc::elect_one()) {
-            tc::mbar_arrive_expect_tx(q_full, AT_TILE);
-            tc::tma_load_2d(q_s, &tma_qkv, q_full, h * ATT_D, row0 + q0);
-            for (int b = 0; b < nblk; ++b) {
-                if (b == 2) tc::mbar_wait(k_free, 0);
-                tc::mbar_arrive_expect_tx(&kv_full[b], 2 * AT_TILE);
-                const int krow = row0 + (kb_first + b) * AT_BK;
-                tc::tma_load_2d(k_s + (b & 1) * AT_TILE, &tma_qkv, &kv_full[b], (p.H + h) * ATT_D, krow);
-                tc::tma_load_2d(v_s + b * AT_TILE, &tma_qkv, &kv_full[b], (2 * p.H + h) * ATT_D, krow);
+    const int qm = lane >> 3, qr = lane & 7;   // ldmatrix.x4: matrix qm, row qr
+    const int quad = lane & 3;
+    const float sc = 0.125f * 1.44269504088896341f;   // 1/sqrt(64) and the base change of exp -> exp2
+    int qi[2];
+    qi[0] = q0 + warp * 16 + (lane >> 2);
+    qi[1] = qi[0] + 8;
+    tc::mbar_wait(q_full, 0);
+    uint32_t qa[ATT_D / 16][4];   // A fragments of this warp's 16 query rows; matrix qm = (row half qm % 2, d half qm / 2)
+#pragma unroll
+    for (int ks = 0; ks < ATT_D / 16; ++ks) {
+        tc::ldmatrix_x4(qa[ks], tc::smem_u32(q_s + tc::sw128_offset(warp * 16 + (qm & 1) * 8 + qr, 2 * ks + (qm >> 1))));
+    }
+    float o[ATT_D / 8][4];
+#pragma unroll
+    for (int dt = 0; dt < ATT_D / 8; ++dt) o[dt][0] = o[dt][1] = o[dt][2] = o[dt][3] = 0.0f;
+    float m_run[2] = {-1e30f, -1e30f}, l_run[2] = {0.0f, 0.0f};
+
+    for (int b = 0; b < nblk; ++b) {
+        const int kb = (kb_first + b) * AT_BK;
+        const uint8_t* kt = k_s + b * AT_TILE;
+        const uint8_t* vt = v_s + b * AT_TILE;
+        // keys of this block visible to each row: j in [lo, hi)
+        int lo[2], hi[2];
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            lo[r] = max(qi[r] - p.win_upper - kb, 0);
+            hi[r] = min(min(qi[r] + p.win_lower + 1 - kb, AT_BK), p.T - kb);
+            if (qi[r] >= p.T) hi[r] = 0;
+        }
+        tc::mbar_wait(&kv_full[b], 0);
+        // S = Q K^T: 16 key tiles of 8; K fragments: matrix qm = (key tile 2 np + qm / 2, d half qm % 2)
+        float sacc[AT_BK / 8][4];
+#pragma unroll
+        for (int nt = 0; nt < AT_BK / 8; ++nt) sacc[nt][0] = sacc[nt][1] = sacc[nt][2] = sacc[nt][3] = 0.0f;
+#pragma unroll
+        for (int ks = 0; ks < ATT_D / 16; ++ks) {
+#pragma unroll
+            for (int np = 0; np < AT_BK / 16; ++np) {
+                uint32_t kf[4];
+                tc::ldmatrix_x4(kf, tc::smem_u32(kt + tc::sw128_offset((2 * np + (qm >> 1)) * 8 + qr, 2 * ks + (qm & 1))));
+                tc::mma_f16_16816(sacc[2 * np], qa[ks], kf[0], kf[1]);
+                tc::mma_f16_16816(sacc[2 * np + 1], qa[ks], kf[2], kf[3]);
             }
         }
-    } else if (warp == 1) {
-        // ---------------- MMA issuer ----------------
-        if (tc::elect_one()) {
-            constexpr uint32_t idesc_s = tc::umma_idesc_f16(128, 128);
-            constexpr uint32_t idesc_o = tc::umma_idesc_f16(128, 64) | (1u << 16);   // B operand MN-major
-            const uint64_t qdesc = tc::umma_desc_sw128(tc::smem_u32(q_s));
-            auto issue_s = [&](int b) {
-                tc::mbar_wait(&kv_full[b], 0);
-                tc::tc_fence_after();
-                const uint64_t kdesc = tc::umma_desc_sw128(tc::smem_u32(k_s + (b & 1) * AT_TILE));
-                const uint32_t tm_s = tmem_base + (uint32_t)((b & 1) * 128);
+        // masked row maxima (a row's 128 keys are spread over the four lanes of its quad)
+        float m_blk[2] = {-1e30f, -1e30f};
 #pragma unroll
-                for (int k = 0; k < ATT_D / 16; ++k) tc::umma_f16(tm_s, qdesc + (uint64_t)(2 * k), kdesc + (uint64_t)(2 * k), idesc_s, k != 0);
-                tc::umma_commit(&s_full[b & 1]);
-            };
-            tc::mbar_wait(q_full, 0);
-            issue_s(0);
-            if (nblk > 2) tc::umma_commit(k_free);   // S_0 done -> K buffer 0 is free for block 2
-            if (nblk > 1) issue_s(1);
-            for (int b = 0; b < nblk; ++b) {
-                const uint32_t tm = tmem_base + (uint32_t)((b & 1) * 128);
-                tc::mbar_wait(&p_ready[b & 1], (uint32_t)((b >> 1) & 1));      // P_b is in tensor memory
-                tc::tc_fence_after();
-                const uint64_t vdesc = umma_desc_sw128_mn(tc::smem_u32(v_s + b * AT_TILE));
+        for (int nt = 0; nt < AT_BK / 8; ++nt) {
 #pragma unroll
-                for (int k = 0; k < AT_BK / 16; ++k) {
-                    // 16 keys = 8 packed TMEM columns of P; 16 rows of V = 2048 B further on
-                    tc::umma_f16_ts(tm + 64u, tm + (uint32_t)(8 * k), vdesc + (uint64_t)((k * 2048) >> 4), idesc_o, k != 0);
-                }
-                tc::umma_commit(&o_full[b & 1]);
-                if (b + 2 < nblk) {
-                    tc::mbar_wait(&buf_free[b & 1], (uint32_t)((b >> 1) & 1));   // the rows have folded O_b in
-                    issue_s(b + 2);
-                }
+            for (int e = 0; e < 4; ++e) {
+                const int r = e >> 1, j = nt * 8 + 2 * quad + (e & 1);
+                if (j >= lo[r] && j < hi[r]) m_blk[r] = fmaxf(m_blk[r], sacc[nt][e]);
             }
         }
-    } else {
-        // ---------------- softmax rows ----------------
-        const int qrt = warp & 3;                    // TMEM lane quarter
-        const int r = qrt * 32 + lane;               // query row within the tile
-        const int qi = q0 + r;
-        const uint32_t lane_sel = (uint32_t)(qrt * 32) << 16;
-        const float sc = 0.125f * 1.44269504088896341f;   // 1/sqrt(64) and the base change of exp -> exp2
-        float o[64];
+        float alpha[2];
 #pragma unroll
-        for (int d = 0; d < 64; ++d) o[d] = 0.0f;
-        float m_run = -1e30f, l_run = 0.0f, alpha_prev = 0.0f;
-        for (int it = 0; it <= nblk; ++it) {
-            float alpha = 0.0f;
-            if (it < nblk) {
-                const int b = it;
-                const uint32_t tm = tmem_base + (uint32_t)((b & 1) * 128);
-                const int kb = (kb_first + b) * AT_BK;
-                // keys of this block visible to this row: j in [lo, hi)
-                int lo = qi - p.win_upper - kb, hi = qi + p.win_lower + 1 - kb;
-                if (lo < 0) lo = 0;
-                if (hi > AT_BK) hi = AT_BK;
-                if (kb + hi > p.T) hi = p.T - kb;
-                if (qi >= p.T) hi = 0;
-                // The window is a band, so per warp (32 consecutive rows) a 32-key column chunk is either invisible to every
-                // row (skipped: no tensor-memory load, no exponentials, P = 0), visible to every row (no per-element masking)
-                // or -- for at most two of the twelve chunks a warp meets -- cut by the band's edge.
-                const int wlo_min = __reduce_min_sync(0xffffffffu, lo), wlo_max = __reduce_max_sync(0xffffffffu, lo);
-                const int whi_min = __reduce_min_sync(0xffffffffu, hi), whi_max = __reduce_max_sync(0xffffffffu, hi);
-                tc::mbar_wait(&s_full[b & 1], (uint32_t)((b >> 1) & 1));
-                tc::tc_fence_after();
-                // pass 1: row maximum over the visible keys (S stays in tensor memory)
-                float m_blk = -1e30f;
-#pragma unroll 1
-                for (int c = 0; c < 4; ++c) {
-                    const int c0 = 32 * c;
-                    if (c0 + 32 <= wlo_min || c0 >= whi_max) continue;
-                    uint32_t v[32];
-                    tc::tmem_ld_32x32(tm + lane_sel + (uint32_t)c0, v);
-                    tc::tmem_ld_wait();
-                    if (c0 >= wlo_max && c0 + 32 <= whi_min) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) m_blk = fmaxf(m_blk, __uint_as_float(v[j]));
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            if (c0 + j >= lo && c0 + j < hi) m_blk = fmaxf(m_blk, __uint_as_float(v[j]));
-                        }
-                    }
-                }
-                const float m_new = fmaxf(m_run, m_blk * sc);
-                alpha = ex2_approx(m_run - m_new);   // 1 when nothing changed, 0 on the first visible block
-                float l_blk = 0.0f;
-                // pass 2: P = exp2(S * sc - m), packed to fp16 pairs, written over the consumed S columns as the A operand of P V
-#pragma unroll 1
-                for (int c = 0; c < 4; ++c) {
-                    const int c0 = 32 * c;
-                    uint32_t pk[16];
-                    if (c0 + 32 <= wlo_min || c0 >= whi_max) {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) pk[j] = 0u;
-                    } else {
-                        uint32_t v[32];
-                        tc::tmem_ld_32x32(tm + lane_sel + (uint32_t)c0, v);
-                        tc::tmem_ld_wait();
-                        if (c0 >= wlo_max && c0 + 32 <= whi_min) {
-#pragma unroll
-                            for (int j = 0; j < 16; ++j) {
-                                const float p0 = ex2_approx(fmaf(__uint_as_float(v[2 * j]), sc, -m_new));
-                                const float p1 = ex2_approx(fmaf(__uint_as_float(v[2 * j + 1]), sc, -m_new));
-                                l_blk += p0 + p1;
-                                const __half2 hp = __floats2half2_rn(p0, p1);
-                                pk[j] = *reinterpret_cast<const uint32_t*>(&hp);
-                            }
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < 16; ++j) {
-                                const int col = c0 + 2 * j;
-                                const float p0 = (col >= lo && col < hi) ? ex2_approx(fmaf(__uint_as_float(v[2 * j]), sc, -m_new)) : 0.0f;
-                                const float p1 = (col + 1 >= lo && col + 1 < hi) ? ex2_approx(fmaf(__uint_as_float(v[2 * j + 1]), sc, -m_new)) : 0.0f;
-                                l_blk += p0 + p1;
-                                const __half2 hp = __floats2half2_rn(p0, p1);
-                                pk[j] = *reinterpret_cast<const uint32_t*>(&hp);
-                            }
-                        }
-                    }
-                    // chunk c of S (columns 32c .. 32c+31) has been read; its P lands in columns 16c .. 16c+15, all consumed
-                    tc::tmem_st_32x16(tm + lane_sel + (uint32_t)(16 * c), pk);
-                }
-                tc::tmem_st_wait();
-                tc::tc_fence_before();
-                __syncwarp();
-                if (lane == 0) tc::mbar_arrive(&p_ready[b & 1]);
-                l_run = l_run * alpha + l_blk;
-                m_run = m_new;
-            }
-            if (it >= 1) {
-                // O = O * alpha_b + P_b V_b for the previous block b = it - 1 (its MMAs ran under this block's softmax)
-                const int b = it - 1;
-                const uint32_t tm = tmem_base + (uint32_t)((b & 1) * 128) + 64u;
-                tc::mbar_wait(&o_full[b & 1], (uint32_t)((b >> 1) & 1));
-                tc::tc_fence_after();
-#pragma unroll
-                for (int c = 0; c < 2; ++c) {
-                    uint32_t v[32];
-                    tc::tmem_ld_32x32(tm + lane_sel + (uint32_t)(32 * c), v);
-                    tc::tmem_ld_wait();
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) o[32 * c + j] = fmaf(o[32 * c + j], alpha_prev, __uint_as_float(v[j]));
-                }
-                tc::tc_fence_before();
-                __syncwarp();
-                if (lane == 0) tc::mbar_arrive(&buf_free[b & 1]);
-            }
-            alpha_prev = alpha;
+        for (int r = 0; r < 2; ++r) {
+            m_blk[r] = fmaxf(m_blk[r], __shfl_xor_sync(0xffffffffu, m_blk[r], 1));
+            m_blk[r] = fmaxf(m_blk[r], __shfl_xor_sync(0xffffffffu, m_blk[r], 2));
+            const float m_new = fmaxf(m_run[r], m_blk[r] * sc);
+            alpha[r] = ex2_approx(m_run[r] - m_new);   // 1 when nothing changed, 0 on the first visible block
+            m_run[r] = m_new;
+            l_run[r] *= alpha[r];
         }
-        if (qi < p.T) {
-            const float inv = l_run > 0.0f ? 1.0f / l_run : 0.0f;
-            uint4* dst = reinterpret_cast<uint4*>(p.out + ((size_t)row0 + qi) * (size_t)(p.H * ATT_D) + (size_t)h * ATT_D);
 #pragma unroll
-            for (int q = 0; q < 8; ++q) {
-                __half2 hh[4];
+        for (int dt = 0; dt < ATT_D / 8; ++dt) {
+            o[dt][0] *= alpha[0]; o[dt][1] *= alpha[0];
+            o[dt][2] *= alpha[1]; o[dt][3] *= alpha[1];
+        }
+        // P = exp2(S * sc - m), then O += P V one 16-key step at a time: P's C fragments of key tiles 2 kk, 2 kk + 1 are
+        // the A fragment of the step; V fragments by ldmatrix.trans, matrix qm = (key half qm % 2, d tile 2 dp + qm / 2)
 #pragma unroll
-                for (int j = 0; j < 4; ++j) hh[j] = __floats2half2_rn(o[8 * q + 2 * j] * inv, o[8 * q + 2 * j + 1] * inv);
-                dst[q] = *reinterpret_cast<uint4*>(hh);
+        for (int kk = 0; kk < AT_BK / 16; ++kk) {
+            float pv[2][4];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int nt = 2 * kk + i;
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int r = e >> 1, j = nt * 8 + 2 * quad + (e & 1);
+                    pv[i][e] = (j >= lo[r] && j < hi[r]) ? ex2_approx(fmaf(sacc[nt][e], sc, -m_run[r])) : 0.0f;
+                }
+                l_run[0] += pv[i][0] + pv[i][1];
+                l_run[1] += pv[i][2] + pv[i][3];
+            }
+            uint32_t pa[4];
+            pa[0] = tc::pack_half2(pv[0][0], pv[0][1]);
+            pa[1] = tc::pack_half2(pv[0][2], pv[0][3]);
+            pa[2] = tc::pack_half2(pv[1][0], pv[1][1]);
+            pa[3] = tc::pack_half2(pv[1][2], pv[1][3]);
+#pragma unroll
+            for (int dp = 0; dp < ATT_D / 16; ++dp) {
+                uint32_t vf[4];
+                tc::ldmatrix_x4_trans(vf, tc::smem_u32(vt + tc::sw128_offset(16 * kk + (qm & 1) * 8 + qr, 2 * dp + (qm >> 1))));
+                tc::mma_f16_16816(o[2 * dp], pa, vf[0], vf[1]);
+                tc::mma_f16_16816(o[2 * dp + 1], pa, vf[2], vf[3]);
             }
         }
     }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tc::tmem_dealloc(tmem_base, 256);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
+        l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
+        if (qi[r] >= p.T) continue;
+        const float inv = l_run[r] > 0.0f ? 1.0f / l_run[r] : 0.0f;
+        __half* dst = p.out + ((size_t)row0 + qi[r]) * (size_t)(p.H * ATT_D) + (size_t)h * ATT_D + 2 * quad;
+#pragma unroll
+        for (int dt = 0; dt < ATT_D / 8; ++dt) {
+            *reinterpret_cast<__half2*>(dst + dt * 8) = __floats2half2_rn(o[dt][2 * r] * inv, o[dt][2 * r + 1] * inv);
+        }
+    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -748,7 +653,7 @@ void TxPlan::run(cudaStream_t stream, ProfileSink* prof) {
             NvtxRange r("MEA");
             constexpr int smem = AT_SMEM;
             ensure_dynamic_smem(tx_attention_tc_kernel, smem);
-            tx_attention_tc_kernel<<<dim3((unsigned)((T + AT_BQ - 1) / AT_BQ), (unsigned)H, (unsigned)N), 192, smem, stream>>>(qkv_map, attn_tc_p);
+            tx_attention_tc_kernel<<<dim3((unsigned)((T + AT_BQ - 1) / AT_BQ), (unsigned)H, (unsigned)N), AT_THREADS, smem, stream>>>(qkv_map, attn_tc_p);
             if (prof) prof->mark("tx_attention", stream);
         }
         {

@@ -1,7 +1,7 @@
 """ctypes binding of libb200call.so (the C ABI in include/b200call.h).
 
-The product path is: this binding -> C ABI -> C++ host (engine.cu) -> sm_100a kernels.  There is no
-CPU fallback: if the shared library is missing, or there is no sm_100 device, calls raise.
+The product path is: this binding -> C ABI -> C++ host (engine.cu) -> sm_90a kernels.  There is no
+CPU fallback: if the shared library is missing, or there is no sm_90 (H100) device, calls raise.
 """
 from __future__ import annotations
 
@@ -15,7 +15,7 @@ from .config import BasecallModelConfig
 
 HERE = pathlib.Path(__file__).resolve().parent
 import os as _os
-# B200CALL_LIB: load another build of the library (A/B comparisons of kernels on the GPU box)
+# B200CALL_LIB: load another build of the library (A/B comparisons of two builds)
 LIB_PATH = pathlib.Path(_os.environ["B200CALL_LIB"]) if _os.environ.get("B200CALL_LIB") else HERE / "libb200call.so"
 
 B200_OK, B200_ERR_INVALID, B200_ERR_CUDA, B200_ERR_UNSUPPORTED, B200_ERR_INTERNAL = 0, -1, -2, -3, -4
@@ -98,7 +98,7 @@ _lib = None
 
 
 def build_library(verbose: bool = False) -> None:
-    """Compile every CUDA source for sm_100a into dorado_b200/libb200call.so (nvcc cross-compiles)."""
+    """Compile every CUDA source for sm_90a into dorado_b200/libb200call.so (nvcc cross-compiles)."""
     subprocess.run(["make", "-j8", "-C", str(HERE / "csrc")], check=True,
                    stdout=None if verbose else subprocess.DEVNULL)
 

@@ -5,7 +5,7 @@
  * last-bit behaviour is platform specific and cannot be reproduced on a GPU.  Because the beam
  * search is full of hard thresholds, "bit-identical" output needs bit-identical transcendentals, so
  * this header pins them: every function below is built only from IEEE-754 binary32 add / mul / fma /
- * div (all correctly rounded on x86-64 and on sm_100a) in a fixed order.  The CUDA kernels
+ * div (all correctly rounded on x86-64 and on sm_90a) in a fixed order.  The CUDA kernels
  * (dorado_b200/csrc/decode.cu) and the CPU oracle (oracle/crf_oracle.c) both include this file, so
  * the two produce the same bits by construction.  Accuracy versus libm: <= 2 ulp over the ranges
  * the decoder uses (tests/test_host_cpu.py::test_numerics_contract_accuracy).

@@ -1,4 +1,4 @@
-/* b200call.h -- C ABI of the B200-native batched basecalling engine (libb200call.so).
+/* b200call.h -- C ABI of the b200call batched basecalling engine (libb200call.so).
  *
  * Drop-in boundary: dorado::basecall::ModelRunnerBase
  * (dorado/basecall/include/basecall/ModelRunnerBase.h:20-38).  The C++ adapter
@@ -10,7 +10,7 @@
  *   Koi                        cmake/Koi.cmake (closed libkoi.a)
  * No C++ types, exceptions or torch types cross this boundary: plain pointers and sizes only.
  * Every function returns B200_OK (0) or a negative b200_status; b200_last_error() gives the message
- * for the calling thread.  The library fails loudly (B200_ERR_CUDA) when no sm_100 device is usable;
+ * for the calling thread.  The library fails loudly (B200_ERR_CUDA) when no sm_90 (H100) device is usable;
  * there is no CPU fallback.
  */
 #ifndef B200CALL_H

@@ -48,7 +48,7 @@ def lstm_layer(x, w_ih, w_hh, b_ih, b_hh, reverse, quant=lambda a: a):
     N, T, C = x.shape
     if reverse:
         x = x[:, ::-1]
-    gx = x @ w_ih.T + (b_ih + b_hh)
+    gx = quant(x @ w_ih.T + (b_ih + b_hh))   # the engine's x-projection GEMM stores gx as fp16
     h = np.zeros((N, C), np.float32)
     c = np.zeros((N, C), np.float32)
     out = np.empty((N, T, C), np.float32)

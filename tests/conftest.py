@@ -18,7 +18,7 @@ MODELS = {
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run on the GPU box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a) GPU")
 
 
 def model_dir(kind: str) -> pathlib.Path:

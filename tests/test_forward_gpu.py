@@ -267,8 +267,8 @@ def test_pool_feeds_every_runner_and_matches_a_single_runner():
 
 
 def test_cluster_shapes_agree():
-    """The hac recurrence runs 16, 32 or 64 chunks per cluster (one or two groups of 16 or 32; chosen from the batch size and
-    the engine's num_runners): the result must not depend on that choice -- bit for bit, fixed and variable chunk sizes --
+    """The hac recurrence runs 16, 32 or 64 chunks per cluster of 8 CTAs (chosen from the batch size and the engine's
+    num_runners): the result must not depend on that choice -- bit for bit, fixed and variable chunk sizes --
     and the 16-chunk shape is the one the other tests pin against the oracle."""
     import os
     from dorado_b200.config import load_model_config
@@ -285,7 +285,7 @@ def test_cluster_shapes_agree():
         for un in (16, 32, 64):
             os.environ["B200_CLUSTER_CHUNKS"] = str(un)
             runner = B200ModelRunner(caller, N, T)
-            assert runner.plan_info()["lstm_rec.chunks_per_cluster"] == un and runner.plan_info()["lstm_rec.ctas"] == N // un * 6
+            assert runner.plan_info()["lstm_rec.chunks_per_cluster"] == un and runner.plan_info()["lstm_rec.ctas"] == N // un * 8
             for i in range(N):
                 runner.accept_chunk(i, sig[i])
             fixed = runner.forward_scores(N).copy()
@@ -364,7 +364,7 @@ def test_variable_chunk_sizes_match_each_chunk_alone(crf_oracle):
 
 
 def test_conv12_tensor_core_kernel_matches_the_fma_kernel_and_the_oracle(monkeypatch):
-    """conv1 + conv2 of the v5 LSTM models: the tcgen05 kernel (conv2 as a 128 x 16 x 80 contraction per tile of 128 samples,
+    """conv1 + conv2 of the v5 LSTM models: the tensor-core kernel (conv2 as a 128 x 16 x 80 mma.sync contraction per tile of 128 samples,
     conv1's output as its fp16 operand) against the fp32 FMA-pipe kernel (B200_CONV12_FMA=1) and against nn_oracle's conv2
     output with the same rounding points.  The conv2 output buffer x2 [N][T + 2 * pad + 8][16] is the first workspace block;
     its padding rows must stay zero.  Ragged T (not a multiple of the 128-sample tile) and several tiles per chunk."""

@@ -88,9 +88,8 @@ def test_full_batch_against_reference(crf_oracle, kind):
     print(f"\n[{kind} N={N} T={T}] scores vs reference fp32 over {rel.size} values: |d|/max(1,|ref|) "
           f"p50 {pct[50]:.2e} p90 {pct[90]:.2e} p99 {pct[99]:.2e} p99.9 {pct[99.9]:.2e} max {rel.max():.2e}; "
           f"within 1e-3: {(rel <= 1e-3).mean():.4f}; rel-L2 {rel_l2:.2e}; max|ref| {scale:.2f}")
-    # fp16 storage of weights, activations and the recurrent state against an fp32 reference.  Measured on B200
-    # (DESIGN.md section 2): rel-L2 2.5e-3 / 1.8e-3 / 1.7e-3, median 1.7e-3 / 1.4e-3 / 1.3e-3, p99 1.3e-2 / 8e-3 / 7e-3,
-    # max 4.3e-2 / 1.7e-2 / 1.4e-2 (fast / hac / sup); the bounds leave a factor ~2
+    # fp16 storage of weights, activations and the recurrent state against an fp32 reference: the error comes from the
+    # fp16 rounding points (DESIGN.md), not from the kernels' accumulation order; the test prints the measured figures
     assert rel_l2 <= 5e-3, rel_l2
     assert pct[50] <= 3e-3 and pct[99] <= 2.5e-2 and rel.max() <= 0.1, (pct, float(rel.max()))
 

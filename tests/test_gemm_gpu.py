@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (dorado_b200/csrc/gemm.cu) vs an fp32 matmul of the same fp16 operands.
+"""wgmma GEMM (dorado_b200/csrc/gemm.cu) vs an fp32 matmul of the same fp16 operands.
 
 Tolerance: the kernel accumulates in fp32 and rounds once to fp16, so |err| <= fp16 half-ulp of the result
 plus accumulation-order noise: rtol 2e-3 (two fp16 ulps), atol 2e-3.

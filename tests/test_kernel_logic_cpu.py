@@ -129,36 +129,22 @@ def test_kmer_neighbour_deduplication():
 
 
 def test_gemm_tile_schedules_cover_every_tile_once():
-    """gemm.cu gemm_tile_at + the grid rule of run_gemm: the default order (shorter dimension fastest) and the two
-    operand-stationary experiment schedules each visit every (row tile, column tile) exactly once."""
-    def tiles_of(cta, grid, m_tiles, n_tiles, wstat, mfast):
+    """gemm.cu gemm_tile_at + the grid rule of run_gemm: the persistent schedule (shorter dimension fastest, CTAs take
+    consecutive tiles, grid = min(tiles, max_ctas)) visits every (row tile, column tile) exactly once."""
+    def tiles_of(cta, grid, m_tiles, n_tiles, mfast):
         i = 0
         while True:
-            if wstat == 1:
-                nt, mt = cta % n_tiles, cta // n_tiles + i * (grid // n_tiles)
-                if mt >= m_tiles:
-                    return
-            elif wstat == 2:
-                mt, nt = cta % m_tiles, cta // m_tiles + i * (grid // m_tiles)
-                if nt >= n_tiles:
-                    return
-            else:
-                tile = cta + i * grid
-                if tile >= m_tiles * n_tiles:
-                    return
-                mt, nt = (tile % m_tiles, tile // m_tiles) if mfast else (tile // n_tiles, tile % n_tiles)
-            yield mt, nt
+            tile = cta + i * grid
+            if tile >= m_tiles * n_tiles:
+                return
+            yield (tile % m_tiles, tile // m_tiles) if mfast else (tile // n_tiles, tile % n_tiles)
             i += 1
 
     for m_tiles, n_tiles in [(12, 3332), (832, 12), (832, 32), (7, 6), (1, 5), (300, 1)]:
-        for max_ctas in (148, 116, 37):
-            for wstat in (0, 1, 2):
-                fixed = {0: 1, 1: n_tiles, 2: m_tiles}[wstat]
-                if wstat and fixed > 74:
-                    continue  # make_gemm_plan does not pick a stationary schedule for such shapes
-                grid = min(m_tiles * n_tiles, max_ctas) if wstat == 0 else max(fixed, (max_ctas // fixed) * fixed)
-                seen = {}
-                for cta in range(grid):
-                    for t in tiles_of(cta, grid, m_tiles, n_tiles, wstat, m_tiles < n_tiles):
-                        seen[t] = seen.get(t, 0) + 1
-                assert len(seen) == m_tiles * n_tiles and set(seen.values()) == {1}, (m_tiles, n_tiles, max_ctas, wstat)
+        for max_ctas in (132, 100, 37):
+            grid = min(m_tiles * n_tiles, max_ctas)
+            seen = {}
+            for cta in range(grid):
+                for t in tiles_of(cta, grid, m_tiles, n_tiles, m_tiles < n_tiles):
+                    seen[t] = seen.get(t, 0) + 1
+            assert len(seen) == m_tiles * n_tiles and set(seen.values()) == {1}, (m_tiles, n_tiles, max_ctas)

@@ -1,6 +1,6 @@
 """The reference-side binding EXECUTED: oracle/_ref/adapter_host is include/B200ModelRunner.h compiled against the reference's
-own headers (ModelRunnerBase, BasecallModelConfig, crf_utils) and libtorch (oracle/Makefile, built where /root/reference
-exists; the binary travels to the GPU box).  It drives the engine only through dorado::basecall::ModelRunnerBase --
+own headers (ModelRunnerBase, BasecallModelConfig, crf_utils) and libtorch (oracle/Makefile `ref`, built by build() where
+the reference sources are available; the binary travels with the tree to the GPU machine).  It drives the engine only through dorado::basecall::ModelRunnerBase --
 accept_chunk(at::Tensor), call_chunks(), sample_stats(), terminate()/restart() -- and must return exactly what the ctypes
 path returns for the same chunks."""
 import pathlib
@@ -22,7 +22,7 @@ def test_cpp_adapter_matches_ctypes_path(tmp_path, kind, batch, chunk, n):
     from dorado_b200.runner import B200Caller, B200ModelRunner
     from dorado_b200.weights import save_b2w, synthetic_weights
     if not HOST.exists():
-        pytest.fail(f"{HOST} is missing: run `make -C oracle ref` where /root/reference exists (it travels with the snapshot)")
+        pytest.fail(f"{HOST} is missing: run `make -C oracle ref` where the reference sources exist (it travels with the tree)")
     cfg = load_model_config(model_dir(kind))
     w = synthetic_weights(cfg, 42)
     T = cfg.normalise_chunk_size(chunk)
