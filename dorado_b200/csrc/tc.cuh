@@ -107,6 +107,16 @@ __device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUte
             ::"r"(smem_u32(smem_dst)), "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
             : "memory");
 }
+// cp.async (LDGSTS): 16 bytes global -> shared, bypassing L1; completion tracked per thread in commit groups, visible to
+// other threads after cp_async_wait and a barrier
+__device__ __forceinline__ void cp_async_16(uint32_t smem_dst, const void* gmem_src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_dst), "l"(gmem_src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// wait until at most N of this thread's cp.async groups are still in flight
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
 // generic-proxy writes (st.shared) -> visible to the async proxy (wgmma / TMA reads of smem)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
