@@ -134,6 +134,19 @@ def load_model_config(path) -> BasecallModelConfig:
             blank_score=float(crf["blank_score"]), qscale=qscale, qbias=qbias, tx=tx)
 
     enc = toml["encoder"]
+    if "type" not in enc:
+        # pre-v4 layout (BasecallModelConfig.cpp:280-295): a fixed swish conv stack described by [encoder] alone; the
+        # defaults of BasecallModelConfig.h apply (5 LSTM layers, a biased CRF linear)
+        stride, C = int(enc["stride"]), int(enc["features"])
+        first = int(enc.get("first_conv_size", 4))
+        features = int(toml["input"]["features"])
+        state_len = toml["global_norm"]["state_len"]
+        convs = [ConvParams(features, first, 5, 1, ACT_SWISH), ConvParams(first, 16, 5, 1, ACT_SWISH),
+                 ConvParams(16, C, 19, stride, ACT_SWISH)]
+        return BasecallModelConfig(
+            name=path.name, path=path, convs=convs, stride=stride, state_len=state_len,
+            outsize=4 ** (state_len + 1), num_features=features, lstm_size=C, lstm_layers=5, bias=True,
+            scale=float(enc["scale"]), blank_score=float(enc["blank_score"]), qscale=qscale, qbias=qbias)
     subs = enc["sublayers"]
     convs = []
     for i, s in enumerate(subs):

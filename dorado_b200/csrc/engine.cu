@@ -486,6 +486,7 @@ b200_result Runner::call_chunks(int num_chunks) {
     B200_CUDA(cudaMemcpyAsync(m_h_out, m_d_out, m_out_bytes, cudaMemcpyDeviceToHost, s));
     B200_CUDA(cudaEventRecord(m_ev[3], s));
     B200_CUDA(cudaStreamSynchronize(s));
+    m_plan->check_errors();
     float h2d = 0, md = 0, d2h = 0;
     B200_CUDA(cudaEventElapsedTime(&h2d, m_ev[0], m_ev[1]));
     B200_CUDA(cudaEventElapsedTime(&md, m_ev[1], m_ev[2]));
@@ -521,6 +522,7 @@ void Runner::step_device(int num_chunks, int iters, float* total_ms, float* forw
         run_decode(num_chunks);
         B200_CUDA(cudaEventRecord(m_ev[2], s));
         B200_CUDA(cudaStreamSynchronize(s));
+        m_plan->check_errors();
         float ms = 0;
         B200_CUDA(cudaEventElapsedTime(&ms, m_ev[0], m_ev[1]));
         fwd += ms;
@@ -565,6 +567,7 @@ void pipelined_steps(Runner** rs, int R, int num_chunks, int iters, float* total
     }
     B200_CUDA(cudaEventRecord(r0.m_ev[1], r0.m_stream));
     B200_CUDA(cudaStreamSynchronize(r0.m_stream));
+    for (int r = 0; r < R; ++r) rs[r]->m_plan->check_errors();
     B200_CUDA(cudaEventElapsedTime(total_ms, r0.m_ev[0], r0.m_ev[1]));
 }
 
@@ -578,6 +581,7 @@ void Runner::forward_scores_to_host(int num_chunks, uint16_t* scores_out) {
     B200_CUDA(cudaMemcpyAsync(scores_out, m_d_scores, (size_t)num_chunks * m_T_out * m_C * sizeof(__half),
                               cudaMemcpyDeviceToHost, s));
     B200_CUDA(cudaStreamSynchronize(s));
+    m_plan->check_errors();
 }
 
 void ProfileSink::begin(cudaStream_t s) { mark("begin", s); }
@@ -615,6 +619,7 @@ std::string Runner::profile(int num_chunks) {
     m_engine.gpu_launches += m_plan->launches();
     run_decode(num_chunks, &sink);
     B200_CUDA(cudaStreamSynchronize(s));
+    m_plan->check_errors();
     std::string out;
     for (auto& kv : sink.report()) out += kv.first + "=" + std::to_string(kv.second) + ";";
     return out;

@@ -65,6 +65,8 @@ public:
     // "key=value;..." facts about the launch plan that measurements need (grid sizes of kernels that deliberately occupy
     // only part of the GPU); empty when every kernel spans the machine
     virtual std::string info() const { return std::string(); }
+    // After the stream has drained: throws if a kernel of the last forward reported a failure through the workspace
+    virtual void check_errors() {}
 };
 
 class Model {

@@ -5,7 +5,8 @@
 //                                                                                         mma.sync; v5 shapes), conv12_kernel (FMA pipe)
 //   ConvStack layer 3      host_linear "cutlass conv"        dorado/nn/ConvStack.cpp:236-275  -> gemm.cu
 //   LSTMStack              host_cutlass_lstm/host_small_lstm dorado/nn/LSTMStack.cpp:127-238 -> lstm_layer_kernel (lstm_size
-//                                                                                         96), gx GEMM + lstm_rec_kernel (192, 384)
+//                                                                                         96), gx GEMM + lstm_rec_kernel (192, 384),
+//                                                                                         gx GEMM + lstm_grid_rec_kernel (768, 1024)
 //   LinearCRF              host_linear                       dorado/nn/CRFModules.cpp:49-122   -> gemm.cu
 // Semantics are those of the CPU modules (ConvStack.cpp:146-163, LSTMStack.cpp:29-41, CRFModules.cpp:24-34).
 //
@@ -631,6 +632,191 @@ __global__ void __launch_bounds__(RecCfg<C, CL, NB>::THREADS, 1) lstm_rec_kernel
 }
 
 // ------------------------------------------------------------------------------------------------
+// lstm_size 768 and 1024: recurrence over a group of CTAs that exchange h through L2 (lstm_grid_rec_kernel).
+//
+// W_hh is 4.5 MiB (768) or 8 MiB (1024) of fp16, more than the registers and shared memory of a cluster, so the weights are
+// spread over a group of G = C / 16 CTAs, one per SM: CTA `rank` owns hidden units [16 rank, 16 rank + 16), i.e. the 64
+// gate rows i, f, g, o of those units (64 x C fp16 = 96 or 128 KiB), in registers for the whole sequence.  Warp w holds
+// the m16 tile of gate w % 4 over K half w / 4 (C / 32 k steps x 4 registers per thread); the two K halves are summed in
+// shared memory.  A group owns NB chunks.  A step is
+//     gx of this thread's cells -> registers    (independent of the recurrence: in flight during the wait)
+//     wait until all G CTAs of the group have arrived after the previous step (counter >= G s)
+//     h_{t-1} of the NB chunks: cp.async.cg (L2, not L1) from the sequence buffer, where the group wrote it
+//     G[64][NB] = W_hh[rows of this CTA] h_{t-1}    mma.sync m16n8k16, B fragments by ldmatrix
+//     gates, cell update (fp32 cell state in registers), h_t (fp16) -> the sequence buffer
+//     arrive: CTA barrier, then one thread: fence + red.release.gpu add 1 on the group's counter
+// h_t goes in place over the layer input x_t, which the x-projection GEMM has consumed; each step writes a new row of the
+// sequence buffer, so one barrier per step orders everything.  The counter wait is bounded: a CTA that waits longer
+// than GR_SPIN_BUDGET cycles, or finds the error word set, sets the error word and returns (the host turns it into an
+// error).  The host launches a grid of whole groups that can all be resident at once (cooperative launch).
+// ------------------------------------------------------------------------------------------------
+constexpr int GR_UNITS = 16;     // hidden units per CTA
+constexpr int GR_THREADS = 256;  // 8 warps: gate = warp % 4, K half = warp / 4
+constexpr long long GR_SPIN_BUDGET = 2000000000LL;  // clock64 cycles: about one second at the H100's 1.98 GHz
+
+struct LstmGridParams {
+    __half* seq;            // [T][N][C] output h (in place over the layer input, which gx has consumed)
+    const __half* gx;       // [T][N][4C]
+    const __half* w_hh;     // [4C][C], PyTorch row order
+    int T, N, reverse;
+    const int32_t* lens;    // optional per-chunk length in samples (variable chunk sizes); stride = samples per step
+    int stride;
+    int n_first;            // first chunk of this launch; group g owns chunks n_first + g NB ..
+    unsigned int* counters; // one arrival counter per group of this launch, zero at launch
+    int* error;             // set to 1 when a group barrier times out
+};
+
+template <int C, int NB>
+struct GridCfg {
+    static constexpr int G = C / GR_UNITS;                 // CTAs per group
+    static constexpr int KS = C / 2 / 16;                  // k steps per warp (one K half)
+    static constexpr int NT = NB / 8;                      // n8 tiles of chunks
+    static constexpr int HS = C + 8;                       // row stride of h (fp16): an ldmatrix phase on distinct banks
+    static constexpr int GS = NB + 4;                      // row stride of the partial gate sums (fp32)
+    static constexpr int PAIRS = GR_UNITS / 2 * NB / GR_THREADS;  // (unit pair, chunk) cells per thread
+    static constexpr size_t SMEM = (size_t)NB * HS * 2 + (size_t)2 * 4 * GR_UNITS * GS * 4;
+    static_assert(C % (2 * 16) == 0 && NT % 2 == 0 && PAIRS >= 1 && (GR_UNITS / 2 * NB) % GR_THREADS == 0, "grid shape");
+};
+
+template <int C, int NB>
+__global__ void __launch_bounds__(GR_THREADS, 1) lstm_grid_rec_kernel(const LstmGridParams p) {
+    using Cfg = GridCfg<C, NB>;
+    constexpr int G = Cfg::G, KS = Cfg::KS, NT = Cfg::NT, HS = Cfg::HS, GS = Cfg::GS, PAIRS = Cfg::PAIRS;
+    constexpr int U = GR_UNITS;
+    extern __shared__ __align__(16) uint8_t smem_raw[];
+    __half* h_s = reinterpret_cast<__half*>(smem_raw);                             // [NB][HS]  h_{t-1}
+    float* g_s = reinterpret_cast<float*>(smem_raw + (size_t)NB * HS * 2);         // [K half][4U gate rows][GS]
+    __shared__ int len_s[NB];
+    __shared__ int abort_s;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int gate = warp & 3, kh = warp >> 2;
+    const int group = (int)blockIdx.x / G, rank = (int)blockIdx.x % G;
+    const int n0 = p.n_first + group * NB;
+    unsigned int* counter = p.counters + group;
+    if (threadIdx.x < NB) len_s[threadIdx.x] = p.lens ? min(p.T, __ldg(p.lens + n0 + threadIdx.x) / p.stride) : p.T;
+
+    // A fragments: W_hh rows gate * C + U rank + lane / 4 (+ 8), columns of K half kh
+    uint32_t a[KS][4];
+    {
+        const __half* w_lo = p.w_hh + (size_t)(gate * C + rank * U + (lane >> 2)) * C + kh * (C / 2);
+        const __half* w_hi = w_lo + (size_t)8 * C;
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+            const int col = ks * 16 + 2 * (lane & 3);
+            a[ks][0] = __ldg(reinterpret_cast<const unsigned int*>(w_lo + col));
+            a[ks][1] = __ldg(reinterpret_cast<const unsigned int*>(w_hi + col));
+            a[ks][2] = __ldg(reinterpret_cast<const unsigned int*>(w_lo + col + 8));
+            a[ks][3] = __ldg(reinterpret_cast<const unsigned int*>(w_hi + col + 8));
+        }
+    }
+    // cells: pair index q = threadIdx.x + j * GR_THREADS -> units (u, u + 1), u = 2 (q % (U / 2)), chunk q / (U / 2)
+    float c_reg[PAIRS][2];
+#pragma unroll
+    for (int j = 0; j < PAIRS; ++j) c_reg[j][0] = c_reg[j][1] = 0.0f;
+    __syncthreads();
+    int steps = 0;
+    for (int i = 0; i < NB; ++i) steps = max(steps, len_s[i]);
+    const int qm = lane >> 3, qr = lane & 7;   // ldmatrix: matrix qm = (n tile qm / 2, k half qm % 2), row qr
+
+    for (int s = 0; s < steps; ++s) {
+        const int t = p.reverse ? steps - 1 - s : s;
+        __half2 gxv[PAIRS][4];
+#pragma unroll
+        for (int j = 0; j < PAIRS; ++j) {
+            const int q = threadIdx.x + j * GR_THREADS;
+            const int u = 2 * (q % (U / 2)), n = q / (U / 2);
+            const __half* gp = p.gx + ((size_t)t * p.N + n0 + n) * (4 * C) + rank * U + u;
+#pragma unroll
+            for (int g = 0; g < 4; ++g) gxv[j][g] = *reinterpret_cast<const __half2*>(gp + g * C);
+        }
+        if (s == 0) {
+            for (int i = threadIdx.x; i < NB * HS / 8; i += GR_THREADS) reinterpret_cast<uint4*>(h_s)[i] = make_uint4(0, 0, 0, 0);
+        } else {
+            // every CTA of the group has stored h_{t-1} (step s - 1)
+            if (threadIdx.x == 0) {
+                const unsigned int target = (unsigned int)(G * s);
+                const long long start = clock64();
+                int failed = 0;
+                while (tc::ld_acquire_gpu(counter) < target) {
+                    if (tc::ld_relaxed_gpu(p.error) != 0 || clock64() - start > GR_SPIN_BUDGET) {
+                        failed = 1;
+                        break;
+                    }
+                }
+                if (failed) atomicExch(p.error, 1);
+                abort_s = failed;
+            }
+            __syncthreads();
+            if (abort_s) return;
+            const int tp = p.reverse ? t + 1 : t - 1;
+            const __half* src = p.seq + ((size_t)tp * p.N + n0) * C;
+            for (int i = threadIdx.x; i < NB * C / 8; i += GR_THREADS) {
+                const int n = i / (C / 8), col = i % (C / 8) * 8;
+                tc::cp_async_16(tc::smem_u32(h_s + n * HS + col), src + (size_t)n * C + col);
+            }
+            tc::cp_async_commit();
+            tc::cp_async_wait<0>();
+        }
+        __syncthreads();
+        float acc[NT][4];
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.0f;
+        const uint32_t hb = tc::smem_u32(h_s) + (uint32_t)(kh * (C / 2) * 2);
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+#pragma unroll
+            for (int np = 0; np < NT / 2; ++np) {
+                uint32_t b[4];
+                const int n = (2 * np + (qm >> 1)) * 8 + qr, k = ks * 16 + (qm & 1) * 8;
+                tc::ldmatrix_x4(b, hb + (uint32_t)((n * HS + k) * 2));
+                tc::mma_f16_16816(acc[2 * np], a[ks], b[0], b[1]);
+                tc::mma_f16_16816(acc[2 * np + 1], a[ks], b[2], b[3]);
+            }
+        }
+        {
+            float* gw = g_s + (kh * 4 * U + gate * U + (lane >> 2)) * GS;
+#pragma unroll
+            for (int nt = 0; nt < NT; ++nt) {
+                const int col = nt * 8 + 2 * (lane & 3);
+                *reinterpret_cast<float2*>(gw + col) = make_float2(acc[nt][0], acc[nt][1]);
+                *reinterpret_cast<float2*>(gw + 8 * GS + col) = make_float2(acc[nt][2], acc[nt][3]);
+            }
+        }
+        __syncthreads();
+#pragma unroll
+        for (int j = 0; j < PAIRS; ++j) {
+            const int q = threadIdx.x + j * GR_THREADS;
+            const int u = 2 * (q % (U / 2)), n = q / (U / 2);
+            // outside the chunk (variable chunk sizes) the state is held at zero: a multiplicative mask, not a branch
+            const float alive = t < len_s[n] ? 1.0f : 0.0f;
+            float hv[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                float pre[4];
+#pragma unroll
+                for (int g = 0; g < 4; ++g) {
+                    const float2 x = __half22float2(gxv[j][g]);
+                    const int row = (g * U + u + e) * GS + n;
+                    pre[g] = (g_s[row] + g_s[4 * U * GS + row]) + (e ? x.y : x.x);
+                }
+                const float ig = gate_act(pre[0], 1.0f), fg = gate_act(pre[1], 1.0f);
+                const float gg = gate_act(pre[2], 2.0f), og = gate_act(pre[3], 1.0f);
+                const float cs = (fg * c_reg[j][e] + ig * gg) * alive;
+                c_reg[j][e] = cs;
+                hv[e] = og * tanh_f(cs) * alive;
+            }
+            *reinterpret_cast<__half2*>(p.seq + ((size_t)t * p.N + n0 + n) * C + rank * U + u) = __floats2half2_rn(hv[0], hv[1]);
+        }
+        // arrive: the CTA's h_t stores precede the release; the barrier also ends every read of h_s and g_s of this step
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            __threadfence();
+            tc::red_release_gpu_add(counter, 1u);
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
 // lstm_size 96 (lstm_layer_kernel): all three with gate rows permuted by lstm_fused_row, W_ih [4C][C].
@@ -643,18 +829,52 @@ struct LstmLayerWeights {
 
 class LstmModel;
 
+// Launch shape of lstm_grid_rec_kernel for a padded batch of Np chunks (a multiple of 32), when max_groups groups fit the
+// GPU at once: NB chunks per group, groups per launch, launches per layer (each launch a whole recurrence over its chunks).
+struct GridShape {
+    int nb, groups, launches;
+};
+GridShape grid_shape(int Np, int max_groups32, int max_groups64, int runners) {
+    GridShape s{};
+    // 64 chunks per group when that still fills every resident group: half the barriers per chunk
+    s.nb = (max_groups64 >= 1 && Np % 64 == 0 && Np / 64 >= max_groups64) ? 64 : 32;
+    const int max_groups = s.nb == 64 ? max_groups64 : max_groups32;
+    const int tiles = Np / s.nb;
+    // with R batches in flight, each batch's recurrence takes ~1/R of the SMs and runs beside the others' kernels
+    s.groups = std::min(tiles, std::max(1, max_groups / std::max(1, runners)));
+    s.launches = (tiles + s.groups - 1) / s.groups;
+    return s;
+}
+
 class LstmPlan final : public ForwardPlan {
 public:
+    ~LstmPlan() override {
+        if (grid_error_host) cudaFreeHost(grid_error_host);
+    }
     void run(cudaStream_t stream, ProfileSink* prof) override;
-    int launches() const override { return 1 + 1 + num_layers * (fused ? 1 : 2) + num_linear; }
+    int launches() const override {
+        return 1 + 1 + num_layers * (fused ? 1 : 1 + (grid ? grid_launches : 1)) + num_linear;
+    }
     std::string info() const override {
         if (fused) return "lstm_layer.ctas=" + std::to_string(rec_ctas);
+        if (grid) {
+            return "lstm_grid.ctas=" + std::to_string(rec_ctas) + ";lstm_grid.groups=" + std::to_string(grid_groups) + ";lstm_grid.chunks_per_group=" +
+                   std::to_string(rec_un) + ";lstm_grid.launches_per_layer=" + std::to_string(grid_launches);
+        }
         return "lstm_rec.ctas=" + std::to_string(rec_ctas) + ";lstm_rec.chunks_per_cluster=" + std::to_string(rec_un);
     }
     void set_chunk_lengths(const int32_t* d_lens) override {
         if (!variable) return;  // the mode exists for the models that run variable chunk sizes only
         conv12.lens = d_lens;
         for (auto& rp : rec_p) rp.lens = d_lens;
+        for (auto& gp : grid_p) gp.lens = d_lens;
+    }
+    void check_errors() override {
+        if (!grid_error_host || *grid_error_host == 0) return;
+        *grid_error_host = 0;
+        B200_CUDA(cudaMemset(grid_p[0].error, 0, sizeof(int)));
+        throw std::runtime_error("lstm_grid_rec_kernel: a group of CTAs did not reach its step barrier within the time "
+                                 "budget; the scores of this batch are invalid");
     }
 
     Conv12Params conv12{};
@@ -671,6 +891,15 @@ public:
     std::vector<GemmPlan> gx_gemm;
     std::vector<LstmRecParams> rec_p;
     void launch_rec(int l, cudaStream_t stream) const;
+    // lstm_size 768 / 1024: gx_gemm + grid_launches lstm_grid_rec_kernel launches per layer (rec_un = chunks per group)
+    bool grid = false;
+    int grid_groups = 0, grid_launches = 0;
+    std::vector<LstmGridParams> grid_p;  // [layer * grid_launches + launch]
+    std::vector<int> grid_launch_ctas;   // per launch (the last one may hold fewer groups)
+    unsigned int* grid_counters = nullptr;
+    size_t grid_counter_bytes = 0;
+    int* grid_error_host = nullptr;      // pinned copy of the error word, written at the end of every forward
+    void launch_grid(int i, cudaStream_t stream) const;
     GemmPlan linear1, linear2;
     int num_layers = 0, num_linear = 1;
     const LstmModel* model = nullptr;
@@ -717,9 +946,9 @@ LstmModel::LstmModel(const b200_model_desc& d, const b200_tensor* tensors, int n
     }
     const int C = d.lstm_size;
     if (C != c3.size) throw std::invalid_argument("last convolution size != lstm_size");
-    if (C != 96 && C != 192 && C != 384) {
+    if (C != 96 && C != 192 && C != 384 && C != 768 && C != 1024) {
         // kernels are instantiated for the sizes of the reference's model zoo this engine covers
-        throw Unsupported("lstm_size " + std::to_string(C) + " is not supported (96, 192 and 384 are)");
+        throw Unsupported("lstm_size " + std::to_string(C) + " is not supported (96, 192, 384, 768 and 1024 are)");
     }
 
     if (d.lstm_layers < 1 || d.lstm_layers > 8) throw std::invalid_argument("bad lstm_layers");
@@ -855,7 +1084,69 @@ size_t LstmModel::workspace_bytes(int N, int T_in) const {
     const size_t seq = (size_t)(T_out + 1) * n_pad(N) * desc.lstm_size * 2 + 4096;
     const size_t mid = desc.out_features > 0 ? (size_t)T_out * n_pad(N) * desc.out_features * 2 + 4096 : 0;
     const size_t gx = desc.lstm_size == FL_C ? 0 : (size_t)T_out * n_pad(N) * 4 * desc.lstm_size * 2 + 4096;
-    return x2 + seq + mid + gx + 4096;  // + the tile counter of conv12_tc_kernel
+    // lstm_grid_rec_kernel: at most one arrival counter per 32 chunks and layer, and the error word
+    const size_t grid = desc.lstm_size > 384 ? (size_t)desc.lstm_layers * (n_pad(N) / 32) * 4 + 256 + 4096 : 0;
+    return x2 + seq + mid + gx + grid + 4096;  // + the tile counter of conv12_tc_kernel
+}
+
+// lstm_grid_rec_kernel<C, nb> and its dynamic shared memory (set as the kernel's limit)
+struct GridKernel {
+    const void* fn;
+    size_t smem;
+};
+template <int C, int NB>
+static GridKernel grid_kernel() {
+    ensure_dynamic_smem(lstm_grid_rec_kernel<C, NB>, (int)GridCfg<C, NB>::SMEM);
+    return {reinterpret_cast<const void*>(lstm_grid_rec_kernel<C, NB>), GridCfg<C, NB>::SMEM};
+}
+static GridKernel grid_kernel(int C, int nb) {
+    switch (C * 100 + nb) {
+        case 76832: return grid_kernel<768, 32>();
+        case 76864: return grid_kernel<768, 64>();
+        case 102432: return grid_kernel<1024, 32>();
+        case 102464: return grid_kernel<1024, 64>();
+        default: throw Unsupported("no grid LSTM recurrence instantiation for this lstm_size");
+    }
+}
+
+// Groups of lstm_grid_rec_kernel that fit the GPU at once: every CTA of a launch must be resident, because CTAs wait for
+// each other at every step.
+static int grid_max_groups(int C, int nb) {
+    int dev = 0, sms = 0, per_sm = 0;
+    B200_CUDA(cudaGetDevice(&dev));
+    B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const GridKernel k = grid_kernel(C, nb);
+    B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k.fn, GR_THREADS, k.smem));
+    return per_sm * sms / (C / GR_UNITS);
+}
+
+// Chunks per group, groups per launch and launches per layer of lstm_size 768 / 1024 (grid_shape); B200_GRID_CHUNKS
+// (32 or 64) and B200_GRID_GROUPS override the choice for tuning and for the tests that compare shapes.
+static void plan_grid(LstmPlan& plan, int C, int Np, int runners) {
+    const int mg32 = grid_max_groups(C, 32), mg64 = grid_max_groups(C, 64);
+    if (mg32 < 1) throw Unsupported("lstm_size " + std::to_string(C) + ": one group of CTAs does not fit this GPU");
+    GridShape s = grid_shape(Np, mg32, mg64, runners);
+    if (const char* e = std::getenv("B200_GRID_CHUNKS")) {
+        const int v = std::atoi(e);
+        if ((v != 32 && v != 64) || Np % v != 0 || (v == 64 && mg64 < 1)) {
+            throw std::invalid_argument("B200_GRID_CHUNKS must be 32 or 64 and divide the padded batch");
+        }
+        s.nb = v;
+        s.groups = std::min(Np / v, std::max(1, (v == 64 ? mg64 : mg32) / std::max(1, runners)));
+    }
+    if (const char* e = std::getenv("B200_GRID_GROUPS")) {
+        const int v = std::atoi(e);
+        if (v < 1 || v > (s.nb == 64 ? mg64 : mg32)) throw std::invalid_argument("B200_GRID_GROUPS must be 1 .. the resident groups");
+        s.groups = std::min(v, Np / s.nb);
+    }
+    s.launches = (Np / s.nb + s.groups - 1) / s.groups;
+    plan.rec_un = s.nb;
+    plan.grid_groups = s.groups;
+    plan.grid_launches = s.launches;
+    plan.rec_ctas = s.groups * (C / GR_UNITS);
+    for (int i = 0; i < s.launches; ++i) {
+        plan.grid_launch_ctas.push_back(std::min(s.groups, Np / s.nb - i * s.groups) * (C / GR_UNITS));
+    }
 }
 
 std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half* signal, __half* scores, void* ws,
@@ -885,6 +1176,13 @@ std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half*
     const bool fused = C == FL_C;
     __half* gxbuf = fused ? nullptr : reinterpret_cast<__half*>(take((size_t)T_out * Np * 4 * C * 2));
     int* tile_counter = reinterpret_cast<int*>(take(256));
+    const bool grid = C > 384;
+    if (grid) {
+        plan->grid = true;
+        plan->grid_counter_bytes = (size_t)desc.lstm_layers * (Np / 32) * sizeof(unsigned int);
+        plan->grid_counters = reinterpret_cast<unsigned int*>(take(plan->grid_counter_bytes));
+    }
+    int* grid_error = grid ? reinterpret_cast<int*>(take(256)) : nullptr;
 
     // conv1 + conv2
     plan->conv12 = Conv12Params{signal, x2, conv_w, N, T_in, Tp, pad3(), desc.convs[0].size, desc.convs[0].winlen,
@@ -893,6 +1191,11 @@ std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half*
     // the v5 shape runs conv2 on the tensor cores (conv12_tc_kernel); anything else keeps the FMA-pipe kernel
     // (B200_CONV12_FMA=1 forces it: the tests compare the two)
     plan->conv12_tc = desc.convs[0].size == 16 && desc.convs[1].winlen == 5 && !std::getenv("B200_CONV12_FMA");
+    if (grid) {
+        B200_CUDA(cudaMemset(grid_error, 0, sizeof(int)));
+        B200_CUDA(cudaHostAlloc(&plan->grid_error_host, sizeof(int), cudaHostAllocDefault));
+        *plan->grid_error_host = 0;
+    }
     plan->conv12_tiles_per_chunk = (T_in + C12_TILE - 1) / C12_TILE;
     {
         const long long tiles = (long long)plan->conv12_tiles_per_chunk * N;
@@ -932,19 +1235,23 @@ std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half*
                     LstmLayerParams{seq, layers[l].w_ih, layers[l].w_hh, layers[l].bias, T_out, Np, l % 2 == 0 ? 1 : 0});
         }
     } else {
-        const int CL = rec_cluster(C);
-        // Chunks per cluster: 32 for large batches, 16 below.  64 chunks (B200_CLUSTER_CHUNKS=64) spill registers next to
-        // the register-resident W_hh of lstm_size 384 and were no faster: hac batch 512, 4 runners, 77.6 vs 77.7 Msamples/s
-        // for 64 vs 32 (two alternating runs each, NVIDIA H100 80GB HBM3 at 700 W).
-        int un = Np > 256 ? 32 : 16;
-        if (const char* e = std::getenv("B200_CLUSTER_CHUNKS")) {   // tuning / A-B override
-            const int v = std::atoi(e);
-            if ((v == 16 || v == 32 || v == 64) && Np % v == 0) un = v;
-            else throw std::invalid_argument("B200_CLUSTER_CHUNKS must be 16, 32 or 64 and divide the padded batch");
+        if (grid) {
+            plan_grid(*plan, C, Np, num_runners_hint);
+        } else {
+            const int CL = rec_cluster(C);
+            // Chunks per cluster: 32 for large batches, 16 below.  64 chunks (B200_CLUSTER_CHUNKS=64) spill registers next to
+            // the register-resident W_hh of lstm_size 384 and were no faster: hac batch 512, 4 runners, 77.6 vs 77.7 Msamples/s
+            // for 64 vs 32 (two alternating runs each, NVIDIA H100 80GB HBM3 at 700 W).
+            int un = Np > 256 ? 32 : 16;
+            if (const char* e = std::getenv("B200_CLUSTER_CHUNKS")) {   // tuning / A-B override
+                const int v = std::atoi(e);
+                if ((v == 16 || v == 32 || v == 64) && Np % v == 0) un = v;
+                else throw std::invalid_argument("B200_CLUSTER_CHUNKS must be 16, 32 or 64 and divide the padded batch");
+            }
+            while (Np % un != 0) un /= 2;
+            plan->rec_un = un;
+            plan->rec_ctas = (Np / un) * CL;
         }
-        while (Np % un != 0) un /= 2;
-        plan->rec_un = un;
-        plan->rec_ctas = (Np / un) * CL;
         // With three or more batches in flight the x-projection GEMMs keep off some SMs, so that another batch's recurrence
         // (several milliseconds of latency chain) can start beside them instead of queueing behind a GEMM that owns every SM.
         const int hint = num_runners_hint < 1 ? 1 : num_runners_hint;
@@ -977,7 +1284,26 @@ std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half*
             rp.reverse = (l % 2 == 0) ? 1 : 0;  // reverse_first = true (CRFModel.cpp:40, LSTMStack.cpp:31-41)
             rp.lens = nullptr;
             rp.stride = desc.stride;
-            plan->rec_p.push_back(rp);
+            if (!grid) {
+                plan->rec_p.push_back(rp);
+                continue;
+            }
+            // grid recurrence: launch i covers groups i * grid_groups .. of rec_un chunks, with counters of its own
+            for (int i = 0; i < plan->grid_launches; ++i) {
+                LstmGridParams gp{};
+                gp.seq = seq;
+                gp.gx = gxbuf;
+                gp.w_hh = layers[l].w_hh;
+                gp.T = T_out;
+                gp.N = Np;
+                gp.reverse = rp.reverse;
+                gp.lens = nullptr;
+                gp.stride = desc.stride;
+                gp.n_first = i * plan->grid_groups * plan->rec_un;
+                gp.counters = plan->grid_counters + (size_t)l * (Np / 32) + (size_t)i * plan->grid_groups;
+                gp.error = grid_error;
+                plan->grid_p.push_back(gp);
+            }
         }
     }
     // linear CRF (+ optional decomposition); rows g = t * Np + n  ->  scores[n][t][:]
@@ -1066,6 +1392,23 @@ void LstmPlan::launch_rec(int l, cudaStream_t stream) const {
     }
 }
 
+// A cooperative launch: the driver refuses a grid whose CTAs cannot all be resident at once instead of starting part of it
+void LstmPlan::launch_grid(int i, cudaStream_t stream) const {
+    const GridKernel k = grid_kernel(model->desc.lstm_size, rec_un);
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3((unsigned)grid_launch_ctas[i % grid_launches], 1, 1);
+    cfg.blockDim = dim3(GR_THREADS, 1, 1);
+    cfg.dynamicSmemBytes = k.smem;
+    cfg.stream = stream;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeCooperative;
+    at[0].val.cooperative = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+    void* args[] = {const_cast<LstmGridParams*>(&grid_p[i])};
+    B200_CUDA(cudaLaunchKernelExC(&cfg, k.fn, args));
+}
+
 void LstmPlan::run(cudaStream_t stream, ProfileSink* prof) {
     {
         NvtxRange r("conv");
@@ -1082,6 +1425,7 @@ void LstmPlan::run(cudaStream_t stream, ProfileSink* prof) {
     }
     {
         NvtxRange lstm_range("lstm_stack");
+        if (grid) B200_CUDA(cudaMemsetAsync(grid_counters, 0, grid_counter_bytes, stream));
         const int nl = debug_layers >= 0 && debug_layers < num_layers ? debug_layers : num_layers;
         for (int l = 0; l < nl; ++l) {
             NvtxRange r("lstm_layer");
@@ -1092,6 +1436,13 @@ void LstmPlan::run(cudaStream_t stream, ProfileSink* prof) {
             }
             run_gemm(gx_gemm[l], stream);
             if (prof) prof->mark("lstm_gx_gemm", stream);
+            if (grid) {
+                for (int i = 0; i < grid_launches; ++i) {
+                    launch_grid(l * grid_launches + i, stream);
+                    if (prof) prof->mark("lstm_grid_rec", stream);
+                }
+                continue;
+            }
             launch_rec(l, stream);
             if (prof) prof->mark("lstm_rec", stream);
         }
@@ -1107,6 +1458,8 @@ void LstmPlan::run(cudaStream_t stream, ProfileSink* prof) {
         run_gemm(linear2, stream);
         if (prof) prof->mark("linear2_gemm", stream);
     }
+    // the error word of the grid recurrence, read by check_errors() once the stream has drained
+    if (grid) B200_CUDA(cudaMemcpyAsync(grid_error_host, grid_p[0].error, sizeof(int), cudaMemcpyDeviceToHost, stream));
     B200_CUDA(cudaGetLastError());
 }
 

@@ -117,6 +117,23 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
+// ---------------------------------------------------------------- grid-scope flags (CTAs that are not in one cluster)
+// Arrival on a counter in global memory: release at GPU scope, so that whatever the arriving thread has observed (with a
+// preceding barrier, the whole CTA's stores) is visible to a thread that acquires the new value.
+__device__ __forceinline__ void red_release_gpu_add(unsigned int* p, unsigned int v) {
+    asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ unsigned int ld_acquire_gpu(const unsigned int* p) {
+    unsigned int v;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ int ld_relaxed_gpu(const int* p) {
+    int v;
+    asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+
 // generic-proxy writes (st.shared) -> visible to the async proxy (wgmma / TMA reads of smem)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 

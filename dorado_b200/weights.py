@@ -71,6 +71,8 @@ def tensor_specs(cfg: BasecallModelConfig) -> "OrderedDict[str, tuple]":
         specs[f"{layer + 1}.linear.weight.tensor"] = (cfg.outsize, cfg.out_features)
     else:
         specs[f"{layer}.linear.weight.tensor"] = (cfg.outsize, C)
+        if cfg.bias:   # pre-v4 models (crf_utils.cpp:82-86: the bias follows the weight whenever the config has one)
+            specs[f"{layer}.linear.bias.tensor"] = (cfg.outsize,)
     return specs
 
 

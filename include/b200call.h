@@ -167,12 +167,12 @@ B200_API int b200_runner_accept_chunk_f32(b200_runner* runner, int32_t chunk_idx
 /* Variable chunk sizes (SURVEY.md 8f row 1; CudaCaller::variable_chunk_sizes, api/runner_creation.cpp:24-42,
  * CudaModelRunner::accept_chunk CudaModelRunner.cpp:21-31, nn/AuxiliaryData.cpp:19-124, CUDADecoder.cpp:35-62,126-147):
  * chunks of different lengths share a batch, so a read's tail is not repeat-padded to chunk_size and the work for it shrinks.
- * b200_runner_variable_chunk_sizes() is 1 for the models the mode exists for (LSTM models with the cluster recurrence:
- * lstm_size 192 / 384); b200_runner_accept_chunk_var_f16 takes `len` samples, a positive multiple of the model stride and
+ * b200_runner_variable_chunk_sizes() is 1 for the models the mode exists for (plain LSTM models of lstm_size 192, 384,
+ * 768 and 1024; not FLSTM); b200_runner_accept_chunk_var_f16 takes `len` samples, a positive multiple of the model stride and
  * <= chunk_size (BasecallerNode wraps a read's tail round to the next stride multiple, BasecallerNode.cpp:408-417).  The
  * reference packs the batch as one [1, C, sum T] row with an (offset, length) table; here every chunk keeps its slot and the
  * kernels read the length table: the convolutions see zero padding at the chunk's own end, the recurrence holds a zero
- * state outside 0 .. len-1 and a cluster only walks the steps one of its chunks is alive in, the decoder scans len/stride
+ * state outside 0 .. len-1 and a cluster (group of CTAs) only walks the steps one of its chunks is alive in, the decoder scans len/stride
  * blocks.  b200_result.n_moves gives the blocks of every row. */
 B200_API int32_t b200_runner_variable_chunk_sizes(const b200_runner* runner);
 B200_API int b200_runner_accept_chunk_var_f16(b200_runner* runner, int32_t chunk_idx, const uint16_t* samples, int64_t len);
