@@ -320,15 +320,35 @@ __device__ __forceinline__ float tanh_f(float v) { return gate_act(v, 2.0f); }
 // registers.  Both weight matrices stay in registers as A fragments (2 tiles x 6 K steps x 4 = 48 registers each).
 //
 // x_t is read in place from the sequence buffer (3 KB of 16 contiguous chunk rows per step), prefetched FL_AHEAD steps
-// ahead into a shared-memory ring by cp.async.  A step s is
-//     W_hh h_{s-1}  (ldmatrix from h_s -> 24 mma.sync) + gx_s  -> gates, cell update, h -> h_s and the sequence buffer
-//     W_ih x_{s+1}  (ldmatrix from the ring -> 24 mma.sync), off the recurrence chain: its accumulators are first read
-//                   after the next barrier, where + bias is rounded to fp16 as the x-projection GEMM of the larger sizes
-//                   rounds gx
-//     prefetch x_{s+FL_AHEAD}, one CTA barrier
-// The barrier publishes h_s to every warp and, with h double-buffered, orders the reads of h_{s-1} before its buffer is
-// overwritten; it also makes the ring slot of step s + 2 (waited for by every thread before it) visible.  Writing h_t over
-// x_t in the sequence buffer is safe: x_t was copied into the ring at least two steps earlier, and no later step reads it.
+// ahead into a shared-memory ring by cp.async.
+//
+// The 16 chunks are 16 independent recurrences, and the two n tiles have accumulators of their own: group A (n tile 0,
+// chunks 0-7) and group B (n tile 1, chunks 8-15).  The groups run half a step apart, so that the tensor cores work on one
+// group while the SFU runs the gate math of the other (one step with a single phase order leaves the tensor pipe idle
+// during the gate math and the SFU idle during the MMAs).  Loop step s is
+//     W_hh h_B(s-1)        ldmatrix of the B rows of h_s -> 12 mma.sync into ah_B, first read after barrier A
+//     gates of A, step s   ah_A + gx_A -> cell update, h_A(s) -> h_s and the sequence buffer.  gx_A is W_ih x_A(s) + bias,
+//                          rounded to fp16 as the x-projection GEMM of the larger sizes rounds gx
+//     W_ih x_A(s+1)        ldmatrix of the A rows of the ring -> 12 mma.sync into ax_A, once the gates of A have read it
+//     barrier A            publishes h_A(s)
+//     W_hh h_A(s)          12 mma.sync into ah_A: the chain of A for step s + 1, first read after barrier B
+//     gates of B, step s;  W_ih x_B(s+1)
+//     prefetch x_{s+FL_AHEAD}; barrier B, which publishes h_B(s) and the ring slot of step s + 2
+// The loop has no branch: the products of step T are computed in the last step and never read.  Nothing inside an
+// accumulator changes order (k steps ascending), so the results do not depend on the schedule.
+//
+// Invariants:
+// - h is ONE tile: the rows of A and B, each group with a single buffer.  Every read of h_X(s-1) and the write of h_X(s)
+//   that overwrites it lie on the two sides of the other group's barrier: W_hh h_B(s-1) is read before barrier A of step
+//   s and h_B(s) is written after it; W_hh h_A(s) is read after barrier A of step s and before barrier B of step s, and
+//   h_A(s+1) is written after that.  The group's own barrier orders the write of h_X(s) before its read.  The prologue
+//   reads h_A(-1) and ends with a CTA barrier of its own, before step 0 writes h_A(0).
+// - ring: the cp.async of loop step s writes the slot of step s - 1.  Both groups read x(s-1) in loop step s - 2, before
+//   its barrier B; the copy is issued after barrier B of step s - 1.
+// - cp.async: before barrier B of loop step s every thread has waited for its copies of steps <= s + 2 (FL_AHEAD - 2
+//   groups may stay in flight), and barrier B makes them visible.  Both groups read x(s+2) in loop step s + 1.
+// - Writing h_t over x_t in the sequence buffer: both groups write h of step s in loop step s.  The copy of x(s) into the
+//   ring completed before barrier B of loop step s - 2, and nothing reads x(s) from the sequence buffer after it.
 // ------------------------------------------------------------------------------------------------
 constexpr int FL_C = 96;
 constexpr int FL_NB = 16;                   // chunks per CTA
@@ -336,10 +356,10 @@ constexpr int FL_THREADS = 32 * FL_C / 8;   // one warp per 8 hidden units
 constexpr int FL_KS = FL_C / 16;            // K steps
 constexpr int FL_HS = FL_C + 8;             // row stride (fp16) of h and x tiles: the 8 rows of an ldmatrix phase on distinct banks
 constexpr int FL_TILE = FL_NB * FL_HS;      // one [chunk][unit] tile
+constexpr int FL_GROUP_BYTES = 8 * FL_HS * 2;   // offset of the rows of group B in a tile
 constexpr int FL_RING = 8;                  // x_t slots
-// Steps between the cp.async of x_t and its use.  Step s copies into the slot of step s - 1, whose x every warp consumed
-// before the barrier that ends step s - 1 at the latest.  The copy has to be complete at the end of step s + FL_AHEAD - 2,
-// so it has FL_AHEAD - 2 steps to land.
+// Steps between the cp.async of x_t and its use.  Step s copies into the slot of step s - 1.  The copy has to be complete
+// at the end of step s + FL_AHEAD - 2, so it has FL_AHEAD - 2 steps to land.
 constexpr int FL_AHEAD = FL_RING - 1;
 constexpr int FL_X_COPIES = FL_NB * FL_C * 2 / 16;   // 16-byte copies per step
 
@@ -356,7 +376,7 @@ struct LstmLayerParams {
 
 __global__ void __launch_bounds__(FL_THREADS, 1) lstm_layer_kernel(const LstmLayerParams p) {
     constexpr int C = FL_C, NB = FL_NB, KS = FL_KS, HS = FL_HS;
-    __shared__ __align__(16) __half h_s[2 * FL_TILE];       // h_{s-1} / h_s
+    __shared__ __align__(16) __half h_s[FL_TILE];            // h of both groups
     __shared__ __align__(16) __half x_s[FL_RING * FL_TILE];  // x_t ring
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n0 = blockIdx.x * NB;
@@ -396,71 +416,71 @@ __global__ void __launch_bounds__(FL_THREADS, 1) lstm_layer_kernel(const LstmLay
     float bias[4];
 #pragma unroll
     for (int g = 0; g < 4; ++g) bias[g] = __ldg(p.bias + lstm_fused_row(g, unit));
-    float c_reg[2][2] = {{0.0f, 0.0f}, {0.0f, 0.0f}};  // [n tile][chunk of the pair]
+    float c_reg[2][2] = {{0.0f, 0.0f}, {0.0f, 0.0f}};  // [group][chunk of the pair]
 
-    const int qm = lane >> 3, qr = lane & 7;  // ldmatrix: matrix qm = (n tile qm / 2, k half qm % 2), row qr
-    const uint32_t frag_off = (uint32_t)((((qm >> 1) * 8 + qr) * HS + (qm & 1) * 8) * 2);
-    // acc[mt][nt] (+)= A[mt] x tile, K = C: the 16 x 4 fragment layout of the gates described above
-    auto mma_tile = [&](float (*acc)[2][4], const uint32_t (*a)[KS][4], uint32_t tile) {
+    // ldmatrix.x4 over two k steps of one group's 8 rows: matrix qm = (k step qm / 2, k half qm % 2), row qr
+    const int qm = lane >> 3, qr = lane & 7;
+    const uint32_t frag_off = (uint32_t)((qr * HS + qm * 8) * 2);
+    const uint32_t h_frag = tc::smem_u32(h_s) + frag_off, x_frag = tc::smem_u32(x_s) + frag_off;
+    // acc[mt] = A[mt] x (the 8 chunk rows at `rows`), K = C in ascending k steps: n tile `group` of the gate layout above
+    auto mma_group = [&](float (*acc)[4], const uint32_t (*a)[KS][4], uint32_t rows) {
 #pragma unroll
-        for (int ks = 0; ks < KS; ++ks) {
+        for (int mt = 0; mt < 2; ++mt) acc[mt][0] = acc[mt][1] = acc[mt][2] = acc[mt][3] = 0.0f;
+#pragma unroll
+        for (int kp = 0; kp < KS / 2; ++kp) {
             uint32_t b[4];
-            tc::ldmatrix_x4(b, tile + frag_off + ks * 32);
+            tc::ldmatrix_x4(b, rows + kp * 64);
 #pragma unroll
-            for (int mt = 0; mt < 2; ++mt) {
-                tc::mma_f16_16816(acc[mt][0], a[mt][ks], b[0], b[1]);
-                tc::mma_f16_16816(acc[mt][1], a[mt][ks], b[2], b[3]);
-            }
+            for (int mt = 0; mt < 2; ++mt) tc::mma_f16_16816(acc[mt], a[mt][2 * kp], b[0], b[1]);
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt) tc::mma_f16_16816(acc[mt], a[mt][2 * kp + 1], b[2], b[3]);
         }
     };
-    float ax[2][2][4];  // W_ih x of the next step
-    auto zero = [](float (*acc)[2][4]) {
+    float ah[2][2][4], ax[2][2][4];  // [group][tile][element]: W_hh h and W_ih x of the group's next gates
+
+    // Gates of group g at one step: gate `gate` of the cell (g, e) is tile gate / 2, row half gate % 2 -> accumulator
+    // element 2 (gate % 2) + e.  ax[g] is read first and then refilled with W_ih x of the next step from ring slot x_next.
+    auto gates = [&](const int g, __half* out, const uint32_t x_next) {
+        float pre[2][4];
 #pragma unroll
-        for (int mt = 0; mt < 2; ++mt)
+        for (int gate = 0; gate < 4; ++gate) {
+            const int mt = gate >> 1, j = 2 * (gate & 1);
+            const float2 gx = __half22float2(__floats2half2_rn(ax[g][mt][j] + bias[gate], ax[g][mt][j + 1] + bias[gate]));
+            pre[0][gate] = ah[g][mt][j] + gx.x;
+            pre[1][gate] = ah[g][mt][j + 1] + gx.y;
+        }
+        mma_group(ax[g], wi, x_next + g * FL_GROUP_BYTES);
 #pragma unroll
-            for (int nt = 0; nt < 2; ++nt) acc[mt][nt][0] = acc[mt][nt][1] = acc[mt][nt][2] = acc[mt][nt][3] = 0.0f;
+        for (int e = 0; e < 2; ++e) {
+            const float ig = gate_act(pre[e][0], 1.0f), fg = gate_act(pre[e][1], 1.0f);
+            const float gg = gate_act(pre[e][2], 2.0f), og = gate_act(pre[e][3], 1.0f);
+            const float cs = fmaf(ig, gg, fg * c_reg[g][e]);  // fused explicitly, so that its rounding is fixed
+            c_reg[g][e] = cs;
+            const __half hv = __float2half_rn(og * tanh_f(cs));
+            const int n = g * 8 + 2 * (lane & 3) + e;
+            h_s[n * HS + unit] = hv;
+            out[(size_t)n * C] = hv;
+        }
     };
     tc::cp_async_wait<FL_AHEAD - 2>();  // x of steps 0 and 1
     __syncthreads();
-    zero(ax);
-    mma_tile(ax, wi, tc::smem_u32(x_s));
+    mma_group(ax[0], wi, x_frag);
+    mma_group(ax[1], wi, x_frag + FL_GROUP_BYTES);
+    mma_group(ah[0], wh, h_frag);  // h_A(-1) = 0
+    __syncthreads();               // every warp has read h_A(-1) before step 0 writes h_A(0) over it
 
     for (int s = 0; s < T; ++s) {
         const int t = p.reverse ? T - 1 - s : s;
-        const int cur = s & 1;
-        float ah[2][2][4];
-        zero(ah);
-        mma_tile(ah, wh, tc::smem_u32(h_s + cur * FL_TILE));
-        __half* h_next = h_s + (cur ^ 1) * FL_TILE + unit;
         __half* out = p.seq + ((size_t)t * p.N + n0) * C + unit;
-#pragma unroll
-        for (int nt = 0; nt < 2; ++nt) {
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                // gate g of this cell: tile g / 2, row half g % 2 -> accumulator element 2 (g % 2) + e
-                float pre[4];
-#pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    const int j = 2 * (g & 1) + e;
-                    pre[g] = ah[g >> 1][nt][j] + __half2float(__float2half_rn(ax[g >> 1][nt][j] + bias[g]));
-                }
-                const float ig = gate_act(pre[0], 1.0f), fg = gate_act(pre[1], 1.0f);
-                const float gg = gate_act(pre[2], 2.0f), og = gate_act(pre[3], 1.0f);
-                const float cs = fg * c_reg[nt][e] + ig * gg;
-                c_reg[nt][e] = cs;
-                const __half hv = __float2half_rn(og * tanh_f(cs));
-                const int n = nt * 8 + 2 * (lane & 3) + e;
-                h_next[n * HS] = hv;
-                out[(size_t)n * C] = hv;
-            }
-        }
-        if (s + 1 < T) {
-            zero(ax);
-            mma_tile(ax, wi, tc::smem_u32(x_s + ((s + 1) % FL_RING) * FL_TILE));
-        }
+        const uint32_t x_next = x_frag + ((s + 1) % FL_RING) * FL_TILE * 2;
+        mma_group(ah[1], wh, h_frag + FL_GROUP_BYTES);
+        gates(0, out, x_next);
+        named_bar_sync(1, FL_THREADS);  // barrier A
+        mma_group(ah[0], wh, h_frag);
+        gates(1, out, x_next);
         prefetch_x(s + FL_AHEAD);
         tc::cp_async_wait<FL_AHEAD - 2>();  // x of step s + 2 has landed (this thread's part)
-        __syncthreads();
+        named_bar_sync(2, FL_THREADS);  // barrier B
     }
 }
 
