@@ -375,3 +375,69 @@ int b200_test_gemm(int32_t device, const uint16_t* a, const uint16_t* b, const f
 }
 
 }  // extern "C"
+
+// ---- modified-base models -------------------------------------------------------------------------------------------
+extern "C" {
+
+int b200_modbase_engine_create(const b200_modbase_desc* desc, const b200_tensor* tensors, int32_t num_tensors, int32_t device,
+                               b200_modbase_engine** out) {
+    return guarded([&] {
+        if (!desc || !tensors || !out) throw std::invalid_argument("b200_modbase_engine_create: null argument");
+        *out = reinterpret_cast<b200_modbase_engine*>(new b200::ModBaseEngine(*desc, tensors, num_tensors, device));
+    });
+}
+
+int b200_modbase_engine_destroy(b200_modbase_engine* e) {
+    return guarded([&] { delete reinterpret_cast<b200::ModBaseEngine*>(e); });
+}
+
+int b200_modbase_runner_create(b200_modbase_engine* e, int32_t batch_size, b200_modbase_runner** out) {
+    return guarded([&] {
+        if (!e || !out) throw std::invalid_argument("b200_modbase_runner_create: null argument");
+        *out = reinterpret_cast<b200_modbase_runner*>(new b200::ModBaseRunner(*reinterpret_cast<b200::ModBaseEngine*>(e), batch_size));
+    });
+}
+
+int b200_modbase_runner_destroy(b200_modbase_runner* r) {
+    return guarded([&] { delete reinterpret_cast<b200::ModBaseRunner*>(r); });
+}
+
+static const b200::ModBaseRunner* mb_runner(const b200_modbase_runner* r) { return reinterpret_cast<const b200::ModBaseRunner*>(r); }
+int32_t b200_modbase_runner_batch_size(const b200_modbase_runner* r) { return r ? mb_runner(r)->batch_size() : 0; }
+int32_t b200_modbase_runner_sig_len(const b200_modbase_runner* r) { return r ? mb_runner(r)->engine().sig_len : 0; }
+int32_t b200_modbase_runner_seq_len(const b200_modbase_runner* r) { return r ? mb_runner(r)->engine().seq_len : 0; }
+int32_t b200_modbase_runner_out_len(const b200_modbase_runner* r) { return r ? mb_runner(r)->engine().out_len : 0; }
+int32_t b200_modbase_runner_num_out(const b200_modbase_runner* r) { return r ? mb_runner(r)->engine().desc().num_out : 0; }
+
+int b200_modbase_runner_accept_chunk(b200_modbase_runner* r, int32_t idx, const uint16_t* signal, int64_t sig_len,
+                                     const int8_t* kmers, int64_t kmer_elems) {
+    return guarded([&] {
+        if (!r) throw std::invalid_argument("b200_modbase_runner_accept_chunk: null runner");
+        reinterpret_cast<b200::ModBaseRunner*>(r)->accept_chunk(idx, signal, sig_len, kmers, kmer_elems);
+    });
+}
+
+int b200_modbase_runner_call_chunks(b200_modbase_runner* r, int32_t num_chunks, const uint16_t** probs) {
+    return guarded([&] {
+        if (!r || !probs) throw std::invalid_argument("b200_modbase_runner_call_chunks: null argument");
+        *probs = reinterpret_cast<b200::ModBaseRunner*>(r)->call_chunks(num_chunks);
+    });
+}
+
+int b200_modbase_runner_profile(b200_modbase_runner* r, char* buf, uint64_t buf_len) {
+    return guarded([&] {
+        if (!r || !buf || buf_len == 0) throw std::invalid_argument("b200_modbase_runner_profile: null argument");
+        const std::string s = reinterpret_cast<b200::ModBaseRunner*>(r)->profile();
+        std::strncpy(buf, s.c_str(), buf_len - 1);
+        buf[buf_len - 1] = '\0';
+    });
+}
+
+int b200_modbase_runner_debug_read_workspace(b200_modbase_runner* r, uint64_t offset, uint64_t bytes, void* dst) {
+    return guarded([&] {
+        if (!r || !dst) throw std::invalid_argument("b200_modbase_runner_debug_read_workspace: null argument");
+        reinterpret_cast<b200::ModBaseRunner*>(r)->debug_read_workspace(offset, bytes, dst);
+    });
+}
+
+}  // extern "C"

@@ -222,6 +222,84 @@ private:
     cudaEvent_t m_ev[4] = {nullptr, nullptr, nullptr, nullptr};
 };
 
+// Modified-base model conv_lstm_v3 (modbase_model.cu): ModBaseEngine holds the weights of one model on one device (the
+// reference's ModBaseCaller model data), ModBaseRunner one batch in flight (ModBaseRunner's input tensors + the forward).
+struct ModBaseLstmWeights {
+    __half* w_ih = nullptr;  // [4C][C padded to 64]
+    __half* w_hh = nullptr;  // [4C][C]
+    float* bias = nullptr;   // [4C] b_ih + b_hh
+};
+
+class ModBaseEngine {
+public:
+    ModBaseEngine(const b200_modbase_desc& desc, const b200_tensor* tensors, int num_tensors, int device);
+    ~ModBaseEngine();
+    ModBaseEngine(const ModBaseEngine&) = delete;
+    ModBaseEngine& operator=(const ModBaseEngine&) = delete;
+    const b200_modbase_desc& desc() const { return m_desc; }
+    int device() const { return m_device; }
+
+    int sig_len = 0;   // signal samples per chunk
+    int seq_len = 0;   // k-mer steps per chunk
+    int t_enc = 0;     // steps of both encoders' outputs
+    int T = 0;         // LSTM steps (merge conv output)
+    int out_len = 0;   // output steps: T x the upsample scale
+    float* sig12_w = nullptr;  // packed sig_conv1 / sig_conv2 (Conv12Params::w)
+    __half* sig3_w = nullptr;  // GEMM weights [size][K], K index = tap * insize + channel
+    float* sig3_b = nullptr;
+    float* seq1_w = nullptr;   // [winlen][insize][16] | bias [16]
+    __half* seq2_w = nullptr;
+    float* seq2_b = nullptr;
+    __half* merge_w = nullptr;
+    float* merge_b = nullptr;
+    ModBaseLstmWeights lstm[2];
+    float* fc_w = nullptr;     // [num_out][C], fp16 values
+    float* fc_b = nullptr;
+    float* up_w = nullptr;     // [sf num_out][num_out] or null
+    float* up_b = nullptr;
+
+private:
+    b200_modbase_desc m_desc;
+    int m_device;
+};
+
+struct ModBasePlan;
+class ModBaseRunner {
+public:
+    ModBaseRunner(ModBaseEngine& engine, int batch_size);
+    ~ModBaseRunner();
+    int batch_size() const { return m_N; }
+    const ModBaseEngine& engine() const { return m_engine; }
+    void accept_chunk(int idx, const uint16_t* signal, int64_t sig_len, const int8_t* kmers, int64_t kmer_elems);
+    // pinned fp16 [num_chunks][out_len * num_out], valid until the next call
+    const uint16_t* call_chunks(int num_chunks);
+    std::string profile();
+    void debug_read_workspace(uint64_t offset, uint64_t bytes, void* dst);
+
+private:
+    void init();
+    void release();
+    void run(ProfileSink* prof);
+    void check_errors();
+
+    ModBaseEngine& m_engine;
+    int m_N;
+    int64_t m_kmer_elems = 0, m_out_elems = 0;
+    cudaStream_t m_stream = nullptr;
+    std::mutex m_mutex;
+    uint16_t* m_h_sig = nullptr;
+    int8_t* m_h_kmers = nullptr;
+    __half* m_h_out = nullptr;
+    int* m_h_error = nullptr;  // pinned copy of the grid recurrence's error word
+    Arena m_arena;
+    void* m_d_ws = nullptr;
+    size_t m_ws_bytes = 0;
+    __half* m_d_sig = nullptr;
+    int8_t* m_d_kmers = nullptr;
+    __half* m_d_out = nullptr;
+    std::unique_ptr<ModBasePlan> m_plan;
+};
+
 // One process, several devices: see pool.cu.
 class Pool {
 public:

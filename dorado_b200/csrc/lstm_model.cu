@@ -17,6 +17,7 @@
 //   scores  [N][T_out][outsize]
 #include "engine.h"
 #include "gemm.h"
+#include "lstm_kernels.h"
 #include "nvtx.h"
 #include "tc.cuh"
 
@@ -38,17 +39,7 @@ namespace {
 // conv1 (1 -> C1, w1) + conv2 (C1 -> 16, w2), both stride 1, fused; fp32 math, fp16 NTC output.
 // ------------------------------------------------------------------------------------------------
 constexpr int CONV_TT = 256;  // output samples per CTA
-constexpr int MAXW = 9;
-
-struct Conv12Params {
-    const __half* x;  // [N][T]
-    __half* out;      // [N][T_pad][16], row r <-> sample r - front_pad
-    const float* w;   // packed: w1 [c1][w1] | b1 [16] | w2 [k][ci][co] (16x16 per tap) | b2 [16]
-    int N, T, T_pad, front_pad;
-    int c1, w1, w2, act1, act2;
-    const int32_t* lens;  // optional per-chunk length in samples (variable chunk sizes): the chunk is zero beyond it
-    int* tile_counter;    // conv12_tc_kernel: next tile to hand out (zeroed on the stream before every launch)
-};
+constexpr int MAXW = kConv12MaxWin;
 
 constexpr int CONV_W_FLOATS = 16 * MAXW + 16 + MAXW * 16 * 16 + 16;
 
@@ -291,6 +282,32 @@ __global__ void __launch_bounds__(C12_THREADS, 4) conv12_tc_kernel(const Conv12P
     }
 }
 
+}  // namespace
+
+// conv1: torch [c1][1][w] -> [c1][w]; conv2: torch [co][ci][k] -> [k][ci][co]
+float* upload_conv12_weights(const b200_tensor& tw, const b200_tensor& tb, const b200_tensor& tw2, const b200_tensor& tb2,
+                             const b200_conv_desc& c1, const b200_conv_desc& c2) {
+    std::vector<float> pk(CONV_W_FLOATS, 0.0f);
+    float* w1 = pk.data();
+    float* b1 = w1 + 16 * MAXW;
+    float* w2 = b1 + 16;
+    float* b2 = w2 + MAXW * 16 * 16;
+    std::memcpy(w1, tw.data, sizeof(float) * (size_t)c1.size * c1.winlen);
+    std::memcpy(b1, tb.data, sizeof(float) * c1.size);
+    for (int co = 0; co < 16; ++co)
+        for (int ci = 0; ci < c2.insize; ++ci)
+            for (int k = 0; k < c2.winlen; ++k)
+                w2[((size_t)k * 16 + ci) * 16 + co] = tw2.data[((size_t)co * c2.insize + ci) * c2.winlen + k];
+    std::memcpy(b2, tb2.data, sizeof(float) * 16);
+    return upload_f32(pk);
+}
+
+void launch_conv12(const Conv12Params& p, cudaStream_t stream) {
+    conv12_kernel<<<dim3((p.T + CONV_TT - 1) / CONV_TT, p.N, 1), CONV_TT, 0, stream>>>(p);
+}
+
+namespace {
+
 // Gate activations on one MUFU.TANH each: sigmoid(v) = 0.5 tanh(0.5 v) + 0.5 (am = 1), tanh(v) (am = 2); FMUL, MUFU.TANH, FFMA.
 // tanh.approx.f32 is good to ~2^-11 -- the rounding h_t gets anyway when it is stored as fp16, and the gates saturate and
 // contract the error.  The same substitution in the swish of the convolutions was rejected, see common.cuh.
@@ -503,14 +520,6 @@ __global__ void __launch_bounds__(FL_THREADS, 1) lstm_layer_kernel(const LstmLay
 // h_t before the MMAs of step t+1 and the reads of h_{t-1} before its buffer is overwritten at step t+1.
 // C = 192 and 384 split over clusters of 4 and 8 CTAs.
 // ------------------------------------------------------------------------------------------------
-struct LstmRecParams {
-    __half* seq;          // [T][N][C] output h (in place over the layer input, which gx has consumed)
-    const __half* gx;     // [T][N][4C]
-    const __half* w_hh;   // [4C][C], PyTorch row order
-    int T, N, reverse;
-    const int32_t* lens;  // optional per-chunk length in samples (variable chunk sizes); stride = samples per step
-    int stride;
-};
 
 // CTAs per cluster for a hidden size: the CTA's W_hh rows (4 C / CL x C fp16) must fit its registers
 __host__ __device__ constexpr int rec_cluster(int C) { return C <= 192 ? 4 : 8; }
@@ -673,18 +682,6 @@ __global__ void __launch_bounds__(RecCfg<C, CL, NB>::THREADS, 1) lstm_rec_kernel
 constexpr int GR_UNITS = 16;     // hidden units per CTA
 constexpr int GR_THREADS = 256;  // 8 warps: gate = warp % 4, K half = warp / 4
 constexpr long long GR_SPIN_BUDGET = 2000000000LL;  // clock64 cycles: about one second at the H100's 1.98 GHz
-
-struct LstmGridParams {
-    __half* seq;            // [T][N][C] output h (in place over the layer input, which gx has consumed)
-    const __half* gx;       // [T][N][4C]
-    const __half* w_hh;     // [4C][C], PyTorch row order
-    int T, N, reverse;
-    const int32_t* lens;    // optional per-chunk length in samples (variable chunk sizes); stride = samples per step
-    int stride;
-    int n_first;            // first chunk of this launch; group g owns chunks n_first + g NB ..
-    unsigned int* counters; // one arrival counter per group of this launch, zero at launch
-    int* error;             // set to 1 when a group barrier times out
-};
 
 template <int C, int NB>
 struct GridCfg {
@@ -973,26 +970,9 @@ LstmModel::LstmModel(const b200_model_desc& d, const b200_tensor* tensors, int n
 
     if (d.lstm_layers < 1 || d.lstm_layers > 8) throw std::invalid_argument("bad lstm_layers");
 
-    // conv1: torch [c1][1][w] -> [c1][w]; conv2: torch [co][ci][k] -> [k][ci][co]
-    {
-        const auto& tw = find_tensor(tensors, n, "0.conv.weight.tensor");
-        const auto& tb = find_tensor(tensors, n, "0.conv.bias.tensor");
-        const auto& tw2 = find_tensor(tensors, n, "1.conv.weight.tensor");
-        const auto& tb2 = find_tensor(tensors, n, "1.conv.bias.tensor");
-        std::vector<float> pk(CONV_W_FLOATS, 0.0f);
-        float* w1 = pk.data();
-        float* b1 = w1 + 16 * MAXW;
-        float* w2 = b1 + 16;
-        float* b2 = w2 + MAXW * 16 * 16;
-        std::memcpy(w1, tw.data, sizeof(float) * (size_t)c1.size * c1.winlen);
-        std::memcpy(b1, tb.data, sizeof(float) * c1.size);
-        for (int co = 0; co < 16; ++co)
-            for (int ci = 0; ci < c2.insize; ++ci)
-                for (int k = 0; k < c2.winlen; ++k)
-                    w2[((size_t)k * 16 + ci) * 16 + co] = tw2.data[((size_t)co * c2.insize + ci) * c2.winlen + k];
-        std::memcpy(b2, tb2.data, sizeof(float) * 16);
-        conv_w = upload_f32(pk);
-    }
+    conv_w = upload_conv12_weights(find_tensor(tensors, n, "0.conv.weight.tensor"), find_tensor(tensors, n, "0.conv.bias.tensor"),
+                                   find_tensor(tensors, n, "1.conv.weight.tensor"), find_tensor(tensors, n, "1.conv.bias.tensor"),
+                                   c1, c2);
     // conv3 as GEMM weights: [C][k*16 + ci], K padded to a multiple of 64
     {
         const auto& tw = find_tensor(tensors, n, "2.conv.weight.tensor");
@@ -1140,9 +1120,20 @@ static int grid_max_groups(int C, int nb) {
     return per_sm * sms / (C / GR_UNITS);
 }
 
+static void plan_grid(LstmPlan& plan, int C, int Np, int runners) {
+    const LstmGridPlan s = plan_lstm_grid(C, Np, runners);
+    plan.rec_un = s.nb;
+    plan.grid_groups = s.groups;
+    plan.grid_launches = s.launches;
+    plan.rec_ctas = s.ctas;
+    plan.grid_launch_ctas = s.launch_ctas;
+}
+
+}  // namespace
+
 // Chunks per group, groups per launch and launches per layer of lstm_size 768 / 1024 (grid_shape); B200_GRID_CHUNKS
 // (32 or 64) and B200_GRID_GROUPS override the choice for tuning and for the tests that compare shapes.
-static void plan_grid(LstmPlan& plan, int C, int Np, int runners) {
+LstmGridPlan plan_lstm_grid(int C, int Np, int runners) {
     const int mg32 = grid_max_groups(C, 32), mg64 = grid_max_groups(C, 64);
     if (mg32 < 1) throw Unsupported("lstm_size " + std::to_string(C) + ": one group of CTAs does not fit this GPU");
     GridShape s = grid_shape(Np, mg32, mg64, runners);
@@ -1160,14 +1151,34 @@ static void plan_grid(LstmPlan& plan, int C, int Np, int runners) {
         s.groups = std::min(v, Np / s.nb);
     }
     s.launches = (Np / s.nb + s.groups - 1) / s.groups;
-    plan.rec_un = s.nb;
-    plan.grid_groups = s.groups;
-    plan.grid_launches = s.launches;
-    plan.rec_ctas = s.groups * (C / GR_UNITS);
+    LstmGridPlan out;
+    out.nb = s.nb;
+    out.groups = s.groups;
+    out.launches = s.launches;
+    out.ctas = s.groups * (C / GR_UNITS);
     for (int i = 0; i < s.launches; ++i) {
-        plan.grid_launch_ctas.push_back(std::min(s.groups, Np / s.nb - i * s.groups) * (C / GR_UNITS));
+        out.launch_ctas.push_back(std::min(s.groups, Np / s.nb - i * s.groups) * (C / GR_UNITS));
     }
+    return out;
 }
+
+// Chunks per cluster: 32 for large batches, 16 below.  64 chunks (B200_CLUSTER_CHUNKS=64) spill registers next to the
+// register-resident W_hh of lstm_size 384 and were no faster: hac batch 512, 4 runners, 77.6 vs 77.7 Msamples/s for 64 vs 32
+// (two alternating runs each, NVIDIA H100 80GB HBM3 at 700 W).
+int lstm_rec_chunks(int Np) {
+    int un = Np > 256 ? 32 : 16;
+    if (const char* e = std::getenv("B200_CLUSTER_CHUNKS")) {   // tuning / A-B override
+        const int v = std::atoi(e);
+        if ((v == 16 || v == 32 || v == 64) && Np % v == 0) un = v;
+        else throw std::invalid_argument("B200_CLUSTER_CHUNKS must be 16, 32 or 64 and divide the padded batch");
+    }
+    while (Np % un != 0) un /= 2;
+    return un;
+}
+
+int lstm_rec_cluster_ctas(int C) { return rec_cluster(C); }
+
+namespace {
 
 std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half* signal, __half* scores, void* ws,
                                                   size_t ws_bytes) {
@@ -1259,16 +1270,7 @@ std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half*
             plan_grid(*plan, C, Np, num_runners_hint);
         } else {
             const int CL = rec_cluster(C);
-            // Chunks per cluster: 32 for large batches, 16 below.  64 chunks (B200_CLUSTER_CHUNKS=64) spill registers next to
-            // the register-resident W_hh of lstm_size 384 and were no faster: hac batch 512, 4 runners, 77.6 vs 77.7 Msamples/s
-            // for 64 vs 32 (two alternating runs each, NVIDIA H100 80GB HBM3 at 700 W).
-            int un = Np > 256 ? 32 : 16;
-            if (const char* e = std::getenv("B200_CLUSTER_CHUNKS")) {   // tuning / A-B override
-                const int v = std::atoi(e);
-                if ((v == 16 || v == 32 || v == 64) && Np % v == 0) un = v;
-                else throw std::invalid_argument("B200_CLUSTER_CHUNKS must be 16, 32 or 64 and divide the padded batch");
-            }
-            while (Np % un != 0) un /= 2;
+            const int un = lstm_rec_chunks(Np);
             plan->rec_un = un;
             plan->rec_ctas = (Np / un) * CL;
         }
@@ -1404,19 +1406,21 @@ static void launch_rec_c(const LstmRecParams& rp, int un, int ctas, cudaStream_t
     }
 }
 
-void LstmPlan::launch_rec(int l, cudaStream_t stream) const {
-    switch (model->desc.lstm_size) {
-        case 192: launch_rec_c<192>(rec_p[l], rec_un, rec_ctas, stream); break;
-        case 384: launch_rec_c<384>(rec_p[l], rec_un, rec_ctas, stream); break;
+}  // namespace
+
+void launch_lstm_rec(int C, int nb, int ctas, const LstmRecParams& p, cudaStream_t stream) {
+    switch (C) {
+        case 192: launch_rec_c<192>(p, nb, ctas, stream); break;
+        case 384: launch_rec_c<384>(p, nb, ctas, stream); break;
         default: throw Unsupported("no LSTM recurrence instantiation for this lstm_size");
     }
 }
 
 // A cooperative launch: the driver refuses a grid whose CTAs cannot all be resident at once instead of starting part of it
-void LstmPlan::launch_grid(int i, cudaStream_t stream) const {
-    const GridKernel k = grid_kernel(model->desc.lstm_size, rec_un);
+void launch_lstm_grid(int C, int nb, int ctas, const LstmGridParams& p, cudaStream_t stream) {
+    const GridKernel k = grid_kernel(C, nb);
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)grid_launch_ctas[i % grid_launches], 1, 1);
+    cfg.gridDim = dim3((unsigned)ctas, 1, 1);
     cfg.blockDim = dim3(GR_THREADS, 1, 1);
     cfg.dynamicSmemBytes = k.smem;
     cfg.stream = stream;
@@ -1425,8 +1429,18 @@ void LstmPlan::launch_grid(int i, cudaStream_t stream) const {
     at[0].val.cooperative = 1;
     cfg.attrs = at;
     cfg.numAttrs = 1;
-    void* args[] = {const_cast<LstmGridParams*>(&grid_p[i])};
+    void* args[] = {const_cast<LstmGridParams*>(&p)};
     B200_CUDA(cudaLaunchKernelExC(&cfg, k.fn, args));
+}
+
+namespace {
+
+void LstmPlan::launch_rec(int l, cudaStream_t stream) const {
+    launch_lstm_rec(model->desc.lstm_size, rec_un, rec_ctas, rec_p[l], stream);
+}
+
+void LstmPlan::launch_grid(int i, cudaStream_t stream) const {
+    launch_lstm_grid(model->desc.lstm_size, rec_un, grid_launch_ctas[i % grid_launches], grid_p[i], stream);
 }
 
 void LstmPlan::run(cudaStream_t stream, ProfileSink* prof) {

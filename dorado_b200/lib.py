@@ -73,6 +73,13 @@ class CalledChunk(C.Structure):
                 ("n_moves", C.c_uint64), ("sequence", C.c_void_p), ("qstring", C.c_void_p), ("n_bases", C.c_uint64)]
 
 
+class ModBaseDesc(C.Structure):
+    """b200_modbase_desc"""
+    _fields_ = [("sig_convs", ConvDesc * 3), ("seq_convs", ConvDesc * 2), ("merge_conv", ConvDesc),
+                ("lstm_size", C.c_int32), ("num_out", C.c_int32), ("upsample_scale", C.c_int32),
+                ("kmer_len", C.c_int32), ("chunk_size", C.c_int32)]
+
+
 class Stats(C.Structure):
     _fields_ = [("batches_called", C.c_int64), ("model_decode_ms", C.c_double), ("h2d_ms", C.c_double),
                 ("d2h_ms", C.c_double), ("gpu_launches", C.c_int64), ("arena_bytes", C.c_int64)]
@@ -92,6 +99,10 @@ EXPORTS = [
     "b200_pool_create", "b200_pool_destroy", "b200_pool_num_runners", "b200_pool_runner", "b200_pool_out_len",
     "b200_pool_runner_info", "b200_pool_call_chunks", "b200_runner_variable_chunk_sizes",
     "b200_runner_accept_chunk_var_f16", "b200_chunk_benchmarks_lookup", "b200_engine_gpu_name",
+    "b200_modbase_engine_create", "b200_modbase_engine_destroy", "b200_modbase_runner_create", "b200_modbase_runner_destroy",
+    "b200_modbase_runner_batch_size", "b200_modbase_runner_sig_len", "b200_modbase_runner_seq_len",
+    "b200_modbase_runner_out_len", "b200_modbase_runner_num_out", "b200_modbase_runner_accept_chunk",
+    "b200_modbase_runner_call_chunks", "b200_modbase_runner_profile", "b200_modbase_runner_debug_read_workspace",
 ]
 
 _lib = None
@@ -170,6 +181,17 @@ def load_library() -> C.CDLL:
     lib.b200_engine_runner_bytes.argtypes = [vp, i32, i32, C.POINTER(u64)]
     lib.b200_engine_benchmark_batch_sizes.argtypes = [vp, i32, i32, i32, C.POINTER(i32), C.POINTER(f32), i32, C.POINTER(i32)]
     lib.b200_select_batch_size.argtypes = [C.POINTER(i32), C.POINTER(f32), i32, i32, i32, f32, C.POINTER(i32)]
+    lib.b200_modbase_engine_create.argtypes = [C.POINTER(ModBaseDesc), C.POINTER(Tensor), i32, i32, C.POINTER(vp)]
+    lib.b200_modbase_engine_destroy.argtypes = [vp]
+    lib.b200_modbase_runner_create.argtypes = [vp, i32, C.POINTER(vp)]
+    lib.b200_modbase_runner_destroy.argtypes = [vp]
+    for fn in ("batch_size", "sig_len", "seq_len", "out_len", "num_out"):
+        getattr(lib, "b200_modbase_runner_" + fn).argtypes = [vp]
+        getattr(lib, "b200_modbase_runner_" + fn).restype = i32
+    lib.b200_modbase_runner_accept_chunk.argtypes = [vp, i32, vp, C.c_int64, vp, C.c_int64]
+    lib.b200_modbase_runner_call_chunks.argtypes = [vp, i32, C.POINTER(C.POINTER(C.c_uint16))]
+    lib.b200_modbase_runner_profile.argtypes = [vp, C.c_char_p, C.c_uint64]
+    lib.b200_modbase_runner_debug_read_workspace.argtypes = [vp, C.c_uint64, C.c_uint64, vp]
     _lib = lib
     return lib
 
@@ -196,6 +218,23 @@ def model_desc_from_config(cfg: BasecallModelConfig) -> ModelDesc:
         d.attn_window_upper, d.attn_window_lower = t.attn_window
         d.upsample_scale, d.max_seq_len = t.upsample_scale, t.max_seq_len
         d.deepnorm_alpha, d.theta, d.tx_crf_scale = t.deepnorm_alpha, t.theta, t.crf_scale
+    return d
+
+
+def modbase_desc_from_config(cfg) -> ModBaseDesc:
+    """b200_modbase_desc of a conv_lstm_v3 ModBaseModelConfig (dorado_b200.config.load_modbase_config)."""
+    if len(cfg.modules.signal_convs) != 3 or len(cfg.modules.sequence_convs) != 2 or len(cfg.modules.lstms) != 2:
+        # the reference's constructor checks (ModBaseModel.cpp:306-315)
+        raise ValueError("ModBaseConvLSTMV3Model expects 3 signal convolutions, 2 sequence convolutions and 2 lstms")
+    d = ModBaseDesc()
+    conv = lambda c: ConvDesc(c.insize, c.size, c.winlen, c.stride, c.activation)
+    for i, c in enumerate(cfg.modules.signal_convs):
+        d.sig_convs[i] = conv(c)
+    for i, c in enumerate(cfg.modules.sequence_convs):
+        d.seq_convs[i] = conv(c)
+    d.merge_conv = conv(cfg.modules.merge_conv)
+    d.lstm_size, d.num_out, d.upsample_scale = cfg.lstm_size, cfg.num_out, cfg.upsample_scale
+    d.kmer_len, d.chunk_size = cfg.kmer_len, cfg.chunk_size
     return d
 
 

@@ -162,3 +162,54 @@ def fold_flstm_weights(cfg: BasecallModelConfig, tensors: Dict[str, np.ndarray])
         else:
             out[name] = w
     return out
+
+
+def modbase_tensor_specs(cfg) -> "OrderedDict[str, tuple]":
+    """Tensors of a conv_lstm_v3 modified-base model in the order load_modbase_conv_lstm_weights reads them
+    (dorado/modbase/nn/ModBaseModel.cpp:49-75), which is also the order of the module's parameters."""
+    m = cfg.modules
+    specs: "OrderedDict[str, tuple]" = OrderedDict()
+    convs = [(f"sig_conv{i + 1}", c) for i, c in enumerate(m.signal_convs)]
+    convs += [(f"seq_conv{i + 1}", c) for i, c in enumerate(m.sequence_convs)]
+    convs.append(("merge_conv1", m.merge_conv))
+    for name, c in convs:
+        specs[f"{name}.weight.tensor"] = (c.size, c.insize, c.winlen)
+        specs[f"{name}.bias.tensor"] = (c.size,)
+    for l, (C, _) in enumerate(m.lstms):
+        p = f"lstm{l + 1}."
+        specs[p + "weight_ih_l0.tensor"] = (4 * C, C)
+        specs[p + "weight_hh_l0.tensor"] = (4 * C, C)
+        specs[p + "bias_ih_l0.tensor"] = (4 * C,)
+        specs[p + "bias_hh_l0.tensor"] = (4 * C,)
+    specs["fc.weight.tensor"] = (m.linear[1], m.linear[0])
+    specs["fc.bias.tensor"] = (m.linear[1],)
+    if m.upsample is not None:
+        size, sf = m.upsample
+        specs["linear_up.linear.weight.tensor"] = (sf * size, size)
+        specs["linear_up.linear.bias.tensor"] = (sf * size,)
+    return specs
+
+
+def synthetic_modbase_weights(cfg, seed: int = 42) -> "OrderedDict[str, np.ndarray]":
+    """Seeded fan-in-uniform weights with gains that keep the encoders' tanh units out of saturation, the LSTM gates
+    lively but contractive (as synthetic_weights does for the basecaller), and the classes' logits a few units apart,
+    so that the softmax is not flat."""
+    rng = np.random.default_rng(seed)
+    out: "OrderedDict[str, np.ndarray]" = OrderedDict()
+    for name, shape in modbase_tensor_specs(cfg).items():
+        if len(shape) == 1:
+            w = (0.1 * rng.uniform(-1, 1, shape)).astype(np.float32)
+        else:
+            bound = 1.0 / np.sqrt(int(np.prod(shape[1:])))
+            gain = 2.0
+            if "weight_ih" in name:
+                gain = 6.0
+            elif "weight_hh" in name:
+                gain = 1.5
+            elif name == "fc.weight.tensor":
+                gain = 16.0
+            elif name.startswith("linear_up"):
+                gain = 1.5
+            w = (gain * bound * rng.uniform(-1, 1, shape)).astype(np.float32)
+        out[name] = np.ascontiguousarray(w)
+    return out

@@ -368,6 +368,69 @@ B200_API int b200_runner_plan_info(const b200_runner* runner, char* buf, uint64_
 /* Debug: copy `bytes` of the runner's forward workspace (device) starting at `offset` to `dst` (host). */
 B200_API int b200_runner_debug_read_workspace(b200_runner* runner, uint64_t offset, uint64_t bytes, void* dst);
 
+/* ---- Modified-base models (conv_lstm_v3) -----------------------------------------------------------------------
+ *
+ * Replaces ModBaseConvLSTMV3CUDAModel (dorado/modbase/nn/ModBaseModel.cpp:435-601) and the tensors of ModBaseRunner /
+ * ModBaseCaller for one model.  The forward is ModBaseConvLSTMV3Model::forward (ModBaseModel.cpp:354-401):
+ *   signal [1][sig_len] fp16 -> sig_convs[0..2];  k-mer one-hot [seq_len][kmer_len * 4] int8 -> seq_convs[0..1];
+ *   concatenate along channels -> merge_conv -> LSTM forward in time -> LSTM reversed in time -> linear (+ bias)
+ *   -> optional LinearUpsample -> softmax over num_out classes, returned as fp16 [out_len][num_out] per chunk.
+ * Every convolution pads by winlen / 2 (ModsConv, ModBaseModel.cpp:91-97), so the encoders give
+ * (len + 2 (winlen / 2) - winlen) / stride + 1 steps, e.g. 101 for 600 samples and the 6mA@v4 shapes. */
+typedef struct b200_modbase_desc {
+    b200_conv_desc sig_convs[3];   /* ModulesParams::signal_convs: 1 -> c1 (<= 16) -> 16 -> C_sig */
+    b200_conv_desc seq_convs[2];   /* ModulesParams::sequence_convs: kmer_len * 4 -> 16 -> C_seq */
+    b200_conv_desc merge_conv;     /* C_sig + C_seq -> lstm_size */
+    int32_t lstm_size;             /* both LSTM layers: 192 or 384 (cluster kernel), 768 or 1024 (grid kernel) */
+    int32_t num_out;               /* linear out_features */
+    int32_t upsample_scale;        /* LinearUpsample scale_factor, 0 = no upsample */
+    int32_t kmer_len;
+    int32_t chunk_size;            /* ContextParams::chunk_size: signal samples per chunk */
+} b200_modbase_desc;
+
+/* Weights named as load_modbase_conv_lstm_weights reads them (ModBaseModel.cpp:49-75): "sig_conv1.weight.tensor", ...,
+ * "lstm1.weight_ih_l0.tensor", ..., "fc.weight.tensor", "fc.bias.tensor", "linear_up.linear.weight.tensor", ... */
+typedef struct b200_modbase_engine b200_modbase_engine;
+typedef struct b200_modbase_runner b200_modbase_runner;
+
+/* LSTM widths without a recurrence instantiation return B200_ERR_UNSUPPORTED. */
+B200_API int b200_modbase_engine_create(const b200_modbase_desc* desc,
+                                        const b200_tensor* tensors,
+                                        int32_t num_tensors,
+                                        int32_t device,
+                                        b200_modbase_engine** out);
+B200_API int b200_modbase_engine_destroy(b200_modbase_engine* engine);
+
+/* Pinned input and output for batch_size chunks, device arena and launch plan; batch_size must be a multiple of 32
+ * (B200_ERR_INVALID otherwise).  Runners of one engine run concurrently, each on its own stream. */
+B200_API int b200_modbase_runner_create(b200_modbase_engine* engine, int32_t batch_size, b200_modbase_runner** out);
+B200_API int b200_modbase_runner_destroy(b200_modbase_runner* runner);
+B200_API int32_t b200_modbase_runner_batch_size(const b200_modbase_runner* runner);
+B200_API int32_t b200_modbase_runner_sig_len(const b200_modbase_runner* runner); /* samples per chunk */
+B200_API int32_t b200_modbase_runner_seq_len(const b200_modbase_runner* runner); /* k-mer steps per chunk */
+B200_API int32_t b200_modbase_runner_out_len(const b200_modbase_runner* runner); /* output steps per chunk */
+B200_API int32_t b200_modbase_runner_num_out(const b200_modbase_runner* runner);
+
+/* ModBaseRunner::accept_chunk (dorado/modbase/ModBaseRunner.cpp:36-87): copy one chunk's signal (fp16 bits, sig_len
+ * samples) and k-mer encoding (int8, seq_len * kmer_len * 4 values) into slot idx.  Any other length returns
+ * B200_ERR_INVALID. */
+B200_API int b200_modbase_runner_accept_chunk(b200_modbase_runner* runner,
+                                              int32_t idx,
+                                              const uint16_t* signal,
+                                              int64_t sig_len,
+                                              const int8_t* kmers,
+                                              int64_t kmer_elems);
+/* ModBaseRunner::call_chunks: H2D of the first num_chunks slots, forward, D2H; blocking.  *probs points at pinned fp16
+ * [num_chunks][out_len * num_out] owned by the runner, valid until its next call. */
+B200_API int b200_modbase_runner_call_chunks(b200_modbase_runner* runner, int32_t num_chunks, const uint16_t** probs);
+/* One forward with a CUDA event after every kernel launch: "name=ms;name=ms;..." (launch order, device milliseconds). */
+B200_API int b200_modbase_runner_profile(b200_modbase_runner* runner, char* buf, uint64_t buf_len);
+/* Debug: copy `bytes` of the forward workspace starting at `offset` to dst.  The workspace starts with the LSTM
+ * sequence buffer, fp16 [T][batch_size][lstm_size] (T = merge conv output steps): the merge conv output until the first
+ * layer runs, then each layer's h.  B200_DEBUG_LSTM_LAYERS=k, set before the runner is created, stops its forwards
+ * after k LSTM layers. */
+B200_API int b200_modbase_runner_debug_read_workspace(b200_modbase_runner* runner, uint64_t offset, uint64_t bytes, void* dst);
+
 /* Kernel-level test hooks (host buffers; used by tests/ only). */
 B200_API int b200_test_gemm(int32_t device, const uint16_t* a /* [M,K] fp16 */, const uint16_t* b /* [N,K] fp16 */,
                             const float* bias /* [N] or NULL */, int32_t M, int32_t N, int32_t K, int32_t activation,
