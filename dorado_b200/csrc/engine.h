@@ -6,6 +6,7 @@
 #include "b200_crf_math.h"
 #include "frontend.h"
 #include "common.cuh"
+#include "lstm_kernels.h"
 
 #include <atomic>
 #include <condition_variable>
@@ -224,12 +225,6 @@ private:
 
 // Modified-base model conv_lstm_v3 (modbase_model.cu): ModBaseEngine holds the weights of one model on one device (the
 // reference's ModBaseCaller model data), ModBaseRunner one batch in flight (ModBaseRunner's input tensors + the forward).
-struct ModBaseLstmWeights {
-    __half* w_ih = nullptr;  // [4C][C padded to 64]
-    __half* w_hh = nullptr;  // [4C][C]
-    float* bias = nullptr;   // [4C] b_ih + b_hh
-};
-
 class ModBaseEngine {
 public:
     ModBaseEngine(const b200_modbase_desc& desc, const b200_tensor* tensors, int num_tensors, int device);
@@ -252,7 +247,7 @@ public:
     float* seq2_b = nullptr;
     __half* merge_w = nullptr;
     float* merge_b = nullptr;
-    ModBaseLstmWeights lstm[2];
+    LstmLayerWeights lstm[2];
     float* fc_w = nullptr;     // [num_out][C], fp16 values
     float* fc_b = nullptr;
     float* up_w = nullptr;     // [sf num_out][num_out] or null
@@ -280,7 +275,6 @@ private:
     void init();
     void release();
     void run(ProfileSink* prof);
-    void check_errors();
 
     ModBaseEngine& m_engine;
     int m_N;
@@ -290,7 +284,6 @@ private:
     uint16_t* m_h_sig = nullptr;
     int8_t* m_h_kmers = nullptr;
     __half* m_h_out = nullptr;
-    int* m_h_error = nullptr;  // pinned copy of the grid recurrence's error word
     Arena m_arena;
     void* m_d_ws = nullptr;
     size_t m_ws_bytes = 0;

@@ -1,14 +1,18 @@
-// Kernels of lstm_model.cu that other models reuse (modbase_model.cu): the fused conv1 + conv2 of a 1-channel signal, and
-// the LSTM recurrences.  An LSTM layer is the x-projection GEMM (gemm.cu, gx = x W_ih^T + b_ih + b_hh, fp16 [T][N][4C])
-// followed by one of the recurrences, which overwrite the sequence buffer [T][N][C] with h in place.
+// Parts of lstm_model.cu that other models reuse (modbase_model.cu): the fused conv1 + conv2 of a 1-channel signal, and
+// the LSTM stack.  The stack owns how LSTM layers are laid out, planned and launched; its callers see neither the
+// recurrence kernels nor their launch shapes, counters or error word.
 #pragma once
 
 #include "b200call.h"
 #include "common.cuh"
+#include "gemm.h"
 
+#include <string>
 #include <vector>
 
 namespace b200 {
+
+struct ProfileSink;
 
 // conv1 (1 -> c1 <= 16 channels, w1) + conv2 (c1 -> 16, w2), both stride 1 with padding winlen / 2, fused on the FMA pipe
 // (conv12_kernel): fp32 math, fp16 NTC output
@@ -27,42 +31,66 @@ float* upload_conv12_weights(const b200_tensor& w1, const b200_tensor& b1, const
                              const b200_conv_desc& c1, const b200_conv_desc& c2);
 void launch_conv12(const Conv12Params& p, cudaStream_t stream);
 
-// lstm_rec_kernel (lstm_size 192 and 384): a thread-block cluster per lstm_rec_chunks() chunks
-struct LstmRecParams {
-    __half* seq;          // [T][N][C] output h (in place over the layer input, which gx has consumed)
-    const __half* gx;     // [T][N][4C]
-    const __half* w_hh;   // [4C][C], PyTorch row order
-    int T, N, reverse;
-    const int32_t* lens;  // optional per-chunk length in samples (variable chunk sizes); stride = samples per step
-    int stride;
+// One LSTM layer's weights on the device.  lstm_size 96 (lstm_layer_kernel): W_ih [4C][C], W_hh and the bias with their
+// gate rows permuted for the fused kernel.  Other sizes: PyTorch gate order (i | f | g | o), W_ih [4C][C padded to a
+// multiple of 64] for the x-projection GEMM.
+struct LstmLayerWeights {
+    __half* w_ih = nullptr;
+    __half* w_hh = nullptr;  // [4C][C]
+    float* bias = nullptr;   // [4C] b_ih + b_hh (fp32)
 };
+// fp32 PyTorch layouts (W_ih and W_hh [4C][C], b_ih and b_hh [4C]) -> the device layout for lstm_size C
+LstmLayerWeights upload_lstm_layer(int C, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh);
+void free_lstm_layer(LstmLayerWeights& w);
 
-// lstm_grid_rec_kernel (lstm_size 768 and 1024): groups of C / 16 CTAs that exchange h through L2
-struct LstmGridParams {
-    __half* seq;            // [T][N][C] output h (in place over the layer input, which gx has consumed)
-    const __half* gx;       // [T][N][4C]
-    const __half* w_hh;     // [4C][C], PyTorch row order
-    int T, N, reverse;
-    const int32_t* lens;    // optional per-chunk length in samples (variable chunk sizes); stride = samples per step
-    int stride;
-    int n_first;            // first chunk of this launch; group g owns chunks n_first + g NB ..
-    unsigned int* counters; // one arrival counter per group of this launch, zero at launch
-    int* error;             // set to 1 when a group barrier times out
+struct LstmStackDesc {
+    int C = 0;                   // lstm_size: 96, 192, 384, 768 or 1024
+    int T = 0;                   // steps
+    int Np = 0;                  // padded batch: a multiple of 16 (lstm_size 96) or 32
+    int stride = 1;              // samples per step, for the chunk lengths of set_chunk_lengths
+    int runners = 1;             // batches in flight: sizes the grid recurrence and caps the x-projection GEMM's CTAs
+    bool reverse_first = false;  // layer 0 (and every other layer after it) runs reversed in time
+    __half* seq = nullptr;       // [T + 1][Np][C]: the first layer's input, overwritten in place with h by every layer
+    const LstmLayerWeights* layers = nullptr;  // kept by the caller for the stack's lifetime
+    int num_layers = 0;
 };
+// The stack's slice of the caller's workspace: gx [T][Np][4C] (not for lstm_size 96), and for 768 / 1024 the group
+// counters and the error word of the grid recurrence
+size_t lstm_stack_workspace_bytes(int C, int num_layers, int T, int Np);
 
-// Chunks per cluster of lstm_rec_kernel for a padded batch of Np chunks (a multiple of 16), and the cluster size
-int lstm_rec_chunks(int Np);
-int lstm_rec_cluster_ctas(int C);
-// Launches lstm_rec_kernel<C, cluster, nb> over `ctas` CTAs; throws Unsupported for a size without an instantiation
-void launch_lstm_rec(int C, int nb, int ctas, const LstmRecParams& p, cudaStream_t stream);
+// Every layer is lstm_layer_kernel (lstm_size 96), or the x-projection GEMM followed by lstm_rec_kernel (192, 384) or by
+// one or more cooperative launches of lstm_grid_rec_kernel (768, 1024).  Built once per batch shape; reads
+// B200_DEBUG_LSTM_LAYERS, B200_CLUSTER_CHUNKS, B200_GRID_CHUNKS and B200_GRID_GROUPS then.
+class LstmStack {
+public:
+    LstmStack(const LstmStackDesc& d, void* ws);  // ws: lstm_stack_workspace_bytes, 256-byte aligned
+    ~LstmStack();
+    LstmStack(const LstmStack&) = delete;
+    LstmStack& operator=(const LstmStack&) = delete;
+    // Enqueues the layers; false if B200_DEBUG_LSTM_LAYERS stopped the stack early (the sequence buffer then holds the
+    // output of that many layers)
+    bool run(cudaStream_t stream, ProfileSink* prof);
+    // Variable chunk sizes: device array of per-chunk lengths in samples (lstm_size 192 and up)
+    void set_chunk_lengths(const int32_t* d_lens) { m_lens = d_lens; }
+    // After the stream has drained: throws if a group of the grid recurrence timed out at its step barrier
+    void check_errors();
+    std::string info() const;  // the launch shape: lstm_layer.*, lstm_rec.* or lstm_grid.* keys
+    int launches() const;      // kernel launches per run
 
-// Launch shape of lstm_grid_rec_kernel for a padded batch of Np chunks (a multiple of 32) with `runners` batches in flight
-struct LstmGridPlan {
-    int nb = 0, groups = 0, launches = 0, ctas = 0;
-    std::vector<int> launch_ctas;  // per launch (the last one may hold fewer groups)
+private:
+    enum class Kind { Layer, Rec, Grid };
+    Kind m_kind = Kind::Layer;
+    LstmStackDesc m_d;
+    int m_debug_layers = -1;  // >= 0: stop after that many layers
+    // chunks per CTA / cluster / group, groups per launch, launches per layer, CTAs per group
+    int m_nb = 0, m_groups = 0, m_launches = 1, m_group_ctas = 1;
+    std::vector<GemmPlan> m_gx_gemm;  // per layer (not for lstm_size 96)
+    __half* m_gx = nullptr;
+    const int32_t* m_lens = nullptr;
+    unsigned int* m_counters = nullptr;  // lstm_size 768 / 1024: Np / 32 per layer, zeroed at the start of every run
+    size_t m_counter_bytes = 0;
+    int* m_error = nullptr;       // set by a group whose step barrier timed out
+    int* m_error_host = nullptr;  // pinned copy, written at the end of every run
 };
-LstmGridPlan plan_lstm_grid(int C, int Np, int runners);
-// One cooperative launch of lstm_grid_rec_kernel<C, nb>
-void launch_lstm_grid(int C, int nb, int ctas, const LstmGridParams& p, cudaStream_t stream);
 
 }  // namespace b200
