@@ -17,8 +17,9 @@
 //                                  chase reads) and the block probability f32 (before the ^0.4 of the qscore; read along the
 //                                  chosen path only)
 //   out     u8    moves/seq/qstr [N][T], n_bases i32 [N]
-// Thread mapping: one thread per state in both scans (two states per thread for S = 1024 in the forward
-// kernel); the forward kernel adds one beam-search warp per chunk that runs one block behind the scan.
+// Thread mapping: state_len 4 and 5: one thread per state in both scans (two states per thread for S = 1024 in the forward
+// kernel); the forward kernel adds one beam-search warp per chunk that runs one block behind the scan.  state_len 3: one warp
+// per chunk runs both scans and the beam search (crf_decode_warp_kernel), many chunks per CTA.
 #include "decode.h"
 
 #include "b200_crf_math.h"
@@ -699,6 +700,194 @@ __global__ void __launch_bounds__(FwdCfg<SL>::THREADS) crf_fwd_beam_kernel(const
 }
 
 // ------------------------------------------------------------------------------------------------
+// Kernels 1 + 2 for state_len 3 (S = 64): one warp owns one chunk for the whole decode but the traceback, and many chunks
+// share a CTA.  Lane l holds states l and l + 32.  The warp runs the backward scan over its chunk (bwd to HBM), then block by
+// block the forward scan, the posterior row and beam_step<3>, handing over through its own shared-memory slot.  There is no
+// CTA-wide barrier, so the chunks per CTA are limited only by registers and shared memory: a runner's decode packs onto
+// about 1/R of the SMs (R batches in flight, Model::num_runners_hint) and leaves the rest to the other runners' kernels,
+// instead of spreading a few issue-starved scan / beam warps over every SM.  The scans' LSE5 formulas, the posterior max and
+// the normaliser's order (two 32-state xor butterflies, then z0 + z1: crf_oracle.c posts_row) are those of the other state
+// lengths, so the results are the same bit for bit.
+// ------------------------------------------------------------------------------------------------
+constexpr int kWarpDecodeMaxChunks = 16;  // chunks (warps) per CTA: 512 threads, up to 128 registers each
+constexpr int kWarpStPitch = 16 + 2;      // backward pass staging pitch, as ScanCfg<3>::PITCH
+
+struct WarpDecodeSmem {
+    __align__(16) float fa[2][64];        // scan guides, ping-pong (backward pass, then forward pass)
+    float st[16 * kWarpStPitch];          // backward pass: score row staged transposed, as in crf_bwd_scan_kernel
+    __align__(16) __half sc_row[256];     // forward pass -> beam_step: clamped scores, guides bwd[t+1], posteriors of block t
+    __align__(16) float bw_row[64];
+    __align__(16) float post_row[64];
+    BeamSmem bs;
+};
+
+__device__ __forceinline__ float4 clamped_scores(const uint2& r, float clamp_val) {
+    const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&r.x));
+    const float2 f1 = __half22float2(*reinterpret_cast<const __half2*>(&r.y));
+    return make_float4(clampf(f0.x, clamp_val), clampf(f0.y, clamp_val), clampf(f1.x, clamp_val), clampf(f1.y, clamp_val));
+}
+
+__global__ void __launch_bounds__(kWarpDecodeMaxChunks * 32, 1) crf_decode_warp_kernel(const __half* __restrict__ scores,
+                                                                                      float* __restrict__ bwd,
+                                                                                      uint2* __restrict__ beam,
+                                                                                      int N,
+                                                                                      int T_pitch,
+                                                                                      float clamp_val,
+                                                                                      float blank,
+                                                                                      int W,
+                                                                                      float log_beam_cut,
+                                                                                      const int32_t* __restrict__ lens,
+                                                                                      int stride) {
+    constexpr int S = Dims<3>::S, C = Dims<3>::C, P4 = S / 4, PITCH = kWarpStPitch;
+    constexpr int RS = C / 4;  // score row stride in uint2: uint2 v of a row holds state v's four scores
+    constexpr int PF = 4;      // backward pass: score rows in flight per lane
+    extern __shared__ __align__(16) unsigned char warp_decode_smem[];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int chunk = blockIdx.x * (blockDim.x >> 5) + w;
+    if (chunk >= N) return;
+    WarpDecodeSmem& sm = reinterpret_cast<WarpDecodeSmem*>(warp_decode_smem)[w];
+    const int T = lens ? min(T_pitch, __ldg(lens + chunk) / stride) : T_pitch;  // variable chunk sizes
+    const uint2* srow = reinterpret_cast<const uint2*>(scores + (size_t)chunk * T_pitch * C);
+    float* brow = bwd + (size_t)chunk * (T_pitch + 1) * S;
+    const int s0 = lane, s1 = lane + 32;  // this lane's states
+
+    // ================= backward scan (CPUDecoder.cpp:69-92) =================
+    // state q + 16 top: successors 4q + j, scores M[t][(4q + j) * 4 + top]; lane l has q = l % 16, top = l / 16 and top + 2
+    {
+        const int q = lane & 15, top = lane >> 4;
+        auto stage = [&](const uint2& r, int v) {  // state v's four scores -> st[(4 (v % 4) + e) * PITCH + v / 4]
+            const float4 f = clamped_scores(r, clamp_val);
+            float* d = &sm.st[4 * (v & 3) * PITCH + (v >> 2)];
+            d[0] = f.x;
+            d[PITCH] = f.y;
+            d[2 * PITCH] = f.z;
+            d[3 * PITCH] = f.w;
+        };
+        uint2 pf[PF][2];
+#pragma unroll
+        for (int k = 0; k < PF; ++k) {
+            const int tt = T - 1 - k;
+            if (tt >= 0) {
+                pf[k][0] = __ldg(srow + (size_t)tt * RS + s0);
+                pf[k][1] = __ldg(srow + (size_t)tt * RS + s1);
+            }
+        }
+        float own0 = 0.0f, own1 = 0.0f;
+        sm.fa[0][s0] = 0.0f;
+        sm.fa[0][s1] = 0.0f;
+        brow[(size_t)T * S + s0] = 0.0f;
+        brow[(size_t)T * S + s1] = 0.0f;
+        int cur = 0;
+        for (int t = T - 1; t >= 0; t -= PF) {
+#pragma unroll
+            for (int k = 0; k < PF; ++k) {
+                const int tt = t - k;
+                if (tt >= 0) {
+                    stage(pf[k][0], s0);
+                    stage(pf[k][1], s1);
+                    if (tt - PF >= 0) {
+                        pf[k][0] = __ldg(srow + (size_t)(tt - PF) * RS + s0);
+                        pf[k][1] = __ldg(srow + (size_t)(tt - PF) * RS + s1);
+                    }
+                    __syncwarp();
+                    const float4 nx = *reinterpret_cast<const float4*>(&sm.fa[cur][4 * q]);
+                    const float* sa = &sm.st[top * PITCH + q];
+                    const float* sb = &sm.st[(top + 2) * PITCH + q];
+                    own0 = b200_lse5(B200_ADD(own0, blank), B200_ADD(nx.x, sa[0]), B200_ADD(nx.y, sa[4 * PITCH]),
+                                     B200_ADD(nx.z, sa[8 * PITCH]), B200_ADD(nx.w, sa[12 * PITCH]));
+                    own1 = b200_lse5(B200_ADD(own1, blank), B200_ADD(nx.x, sb[0]), B200_ADD(nx.y, sb[4 * PITCH]),
+                                     B200_ADD(nx.z, sb[8 * PITCH]), B200_ADD(nx.w, sb[12 * PITCH]));
+                    sm.fa[cur ^ 1][s0] = own0;
+                    sm.fa[cur ^ 1][s1] = own1;
+                    brow[(size_t)tt * S + s0] = own0;
+                    brow[(size_t)tt * S + s1] = own1;
+                    __syncwarp();  // this block's reads of st / fa come before the next block's writes
+                    cur ^= 1;
+                }
+            }
+        }
+    }
+    __syncwarp();  // every lane's bwd rows are visible to the whole warp (plain loads below: the rows were written here)
+
+    // ================= forward scan + posteriors + beam search =================
+    uint32_t* meta_out = reinterpret_cast<uint32_t*>(beam) + (size_t)chunk * T_pitch * kBeamW;
+    float* prob_out = reinterpret_cast<float*>(beam) + ((size_t)N + chunk) * T_pitch * kBeamW;
+    sm.fa[0][s0] = 0.0f;
+    sm.fa[0][s1] = 0.0f;
+    sm.bw_row[s0] = brow[s0];
+    sm.bw_row[s1] = brow[s1];
+    __syncwarp();
+    BeamLane me{0u, 0u, 0.0f};
+    int width = beam_init<3>(sm.bw_row, sm.bs, me, W, lane);
+    // block t+1's scores and guides are loaded while block t is computed (a block's scan + beam step is far longer than a load)
+    uint2 r0n{}, r1n{};
+    float b0n = 0.0f, b1n = 0.0f;
+    if (T > 0) {
+        r0n = __ldg(srow + s0);
+        r1n = __ldg(srow + s1);
+        b0n = brow[S + s0];
+        b1n = brow[S + s1];
+    }
+    float f0 = 0.0f, f1 = 0.0f;
+    int cur = 0;
+    const int p0 = s0 >> 2, p1 = s1 >> 2;  // predecessors of state s: s / 4 + 16 k
+    for (int t = 0; t < T; ++t) {
+        const uint2 r0 = r0n, r1 = r1n;
+        const float bw0 = b0n, bw1 = b1n;
+        if (t + 1 < T) {
+            r0n = __ldg(srow + (size_t)(t + 1) * RS + s0);
+            r1n = __ldg(srow + (size_t)(t + 1) * RS + s1);
+            b0n = brow[(size_t)(t + 2) * S + s0];
+            b1n = brow[(size_t)(t + 2) * S + s1];
+        }
+        const float4 c0 = clamped_scores(r0, clamp_val), c1 = clamped_scores(r1, clamp_val);
+        {  // clamped scores for the beam step (clamping fp16 values is exact in fp16)
+            const __half2 h00 = __floats2half2_rn(c0.x, c0.y), h01 = __floats2half2_rn(c0.z, c0.w);
+            const __half2 h10 = __floats2half2_rn(c1.x, c1.y), h11 = __floats2half2_rn(c1.z, c1.w);
+            *reinterpret_cast<uint2*>(&sm.sc_row[4 * s0]) =
+                    make_uint2(*reinterpret_cast<const uint32_t*>(&h00), *reinterpret_cast<const uint32_t*>(&h01));
+            *reinterpret_cast<uint2*>(&sm.sc_row[4 * s1]) =
+                    make_uint2(*reinterpret_cast<const uint32_t*>(&h10), *reinterpret_cast<const uint32_t*>(&h11));
+        }
+        sm.bw_row[s0] = bw0;
+        sm.bw_row[s1] = bw1;
+        const float* fc = sm.fa[cur];
+        f0 = b200_lse5(B200_ADD(f0, blank), B200_ADD(fc[p0], c0.x), B200_ADD(fc[p0 + P4], c0.y), B200_ADD(fc[p0 + 2 * P4], c0.z),
+                       B200_ADD(fc[p0 + 3 * P4], c0.w));
+        f1 = b200_lse5(B200_ADD(f1, blank), B200_ADD(fc[p1], c1.x), B200_ADD(fc[p1 + P4], c1.y), B200_ADD(fc[p1 + 2 * P4], c1.z),
+                       B200_ADD(fc[p1 + 3 * P4], c1.w));
+        sm.fa[cur ^ 1][s0] = f0;
+        sm.fa[cur ^ 1][s1] = f1;
+        const float v0 = B200_ADD(f0, bw0), v1 = B200_ADD(f1, bw1);  // fwd + bwd
+        const float mx = warp_max(b200_fmaxf(v0, v1));
+        const float e0 = b200_expf_nonpos(B200_SUB(v0, mx)), e1 = b200_expf_nonpos(B200_SUB(v1, mx));
+        // normaliser in the contract's order: xor butterfly over states 0..31, the same over 32..63, then the two groups
+        float z0 = e0, z1 = e1;
+#pragma unroll
+        for (int o = 16; o >= 1; o >>= 1) {
+            z0 = B200_ADD(z0, __shfl_xor_sync(0xffffffffu, z0, o));
+            z1 = B200_ADD(z1, __shfl_xor_sync(0xffffffffu, z1, o));
+        }
+        const float z = B200_ADD(z0, z1);
+        sm.post_row[s0] = B200_DIV(e0, z);
+        sm.post_row[s1] = B200_DIV(e1, z);
+        __syncwarp();
+        // beam_step ends in a __syncwarp: the next block's writes above come after its reads of this block's rows
+        width = beam_step<3>(sm.sc_row, sm.bw_row, sm.post_row, sm.bs, me, width, W, log_beam_cut, blank, t == T - 1,
+                             meta_out + (size_t)t * kBeamW, prob_out + (size_t)t * kBeamW, lane, nullptr);
+        cur ^= 1;
+    }
+}
+
+// Chunks per CTA of crf_decode_warp_kernel: R batches in flight share the GPU, so one batch's decode is packed onto about
+// 1/R of the SMs (the LSTM layers' grids are sized the same way).
+int warp_decode_chunks_per_cta(int N, int runners) {
+    const int R = runners > 1 ? runners : 1;
+    const int per = (int)(((long long)N * R + kNumSMs - 1) / kNumSMs);
+    return per < 1 ? 1 : (per > kWarpDecodeMaxChunks ? kWarpDecodeMaxChunks : per);
+}
+
+// ------------------------------------------------------------------------------------------------
 // Kernel 3: traceback + sequence / qstring generation (beam_search.cpp:447-455, :54-102).
 // One warp per chunk.  The pointer chase only needs the 4-byte (state, prev, stay) words, so the beam history is two planes
 // (meta, prob) and the chase streams the meta plane alone, in tiles of 32 blocks: while lane 0 walks one tile in shared
@@ -820,6 +1009,33 @@ __global__ void __launch_bounds__(kTbWarps * 32) crf_traceback_kernel(const uint
 
 size_t traceback_smem_bytes(int T) { return kTbWarps * traceback_warp_bytes(T); }
 
+void launch_traceback(const DecodeArgs& a, cudaStream_t stream, ProfileSink* prof) {
+    const size_t smem = traceback_smem_bytes(a.T);
+    if (smem > 48 * 1024) ensure_dynamic_smem(crf_traceback_kernel, 200 * 1024);
+    const int grid = (a.N + kTbWarps - 1) / kTbWarps;
+    NvtxRange r("decode");
+    const uint32_t* meta = reinterpret_cast<const uint32_t*>(a.beam);
+    const float* prob = reinterpret_cast<const float*>(a.beam) + (size_t)a.N * a.T * kBeamW;
+    crf_traceback_kernel<<<grid, kTbWarps * 32, smem, stream>>>(meta, prob, a.N, a.T, a.lens, a.stride, a.qtable, a.moves,
+                                                                a.sequence, a.qstring, a.n_bases);
+    if (prof) prof->mark("crf_traceback", stream);
+}
+
+void launch_decode_warp(const DecodeArgs& a, cudaStream_t stream, ProfileSink* prof) {
+    {
+        const int cpc = warp_decode_chunks_per_cta(a.N, a.runners);
+        const int grid = (a.N + cpc - 1) / cpc;
+        const size_t smem = (size_t)cpc * sizeof(WarpDecodeSmem);
+        ensure_dynamic_smem(crf_decode_warp_kernel, (int)(kWarpDecodeMaxChunks * sizeof(WarpDecodeSmem)));
+        NvtxRange r("beam_search");  // backward scan, forward scan, posteriors and beam search of each chunk in one warp
+        crf_decode_warp_kernel<<<grid, cpc * 32, smem, stream>>>(a.scores, a.bwd, a.beam, a.N, a.T, a.clamp_val, a.blank,
+                                                                 a.beam_width, a.log_beam_cut, a.lens, a.stride);
+        if (prof) prof->mark("crf_fwd_beam", stream);
+    }
+    launch_traceback(a, stream, prof);
+    B200_CUDA(cudaGetLastError());
+}
+
 template <int SL>
 void launch_decode(const DecodeArgs& a, cudaStream_t stream, ProfileSink* prof) {
     {
@@ -838,17 +1054,7 @@ void launch_decode(const DecodeArgs& a, cudaStream_t stream, ProfileSink* prof) 
                                                                    a.beam_width, a.log_beam_cut, a.lens, a.stride, a.dbg);
         if (prof) prof->mark("crf_fwd_beam", stream);
     }
-    {
-        const size_t smem = traceback_smem_bytes(a.T);
-        if (smem > 48 * 1024) ensure_dynamic_smem(crf_traceback_kernel, 200 * 1024);
-        const int grid = (a.N + kTbWarps - 1) / kTbWarps;
-        NvtxRange r("decode");
-        const uint32_t* meta = reinterpret_cast<const uint32_t*>(a.beam);
-        const float* prob = reinterpret_cast<const float*>(a.beam) + (size_t)a.N * a.T * kBeamW;
-        crf_traceback_kernel<<<grid, kTbWarps * 32, smem, stream>>>(meta, prob, a.N, a.T, a.lens, a.stride, a.qtable, a.moves,
-                                                                    a.sequence, a.qstring, a.n_bases);
-        if (prof) prof->mark("crf_traceback", stream);
-    }
+    launch_traceback(a, stream, prof);
     B200_CUDA(cudaGetLastError());
 }
 
@@ -869,6 +1075,8 @@ size_t decode_scratch_bytes(int N, int T, int state_len, size_t* bwd_bytes, size
     return b1 + b2;
 }
 
+int decode_launches(int state_len) { return state_len == 3 ? 2 : 3; }
+
 void decode_scores(const DecodeArgs& a, cudaStream_t stream, ProfileSink* prof) {
     if (a.beam_width < 1 || a.beam_width > kBeamW) {
         throw std::invalid_argument("b200 decode: beam_width must be in [1, 32]");
@@ -883,7 +1091,7 @@ void decode_scores(const DecodeArgs& a, cudaStream_t stream, ProfileSink* prof) 
                                     "holds in shared memory (about 10 700); use a smaller chunk size");
     }
     switch (a.state_len) {
-        case 3: launch_decode<3>(a, stream, prof); break;
+        case 3: launch_decode_warp(a, stream, prof); break;
         case 4: launch_decode<4>(a, stream, prof); break;
         case 5: launch_decode<5>(a, stream, prof); break;
         default: throw std::invalid_argument("b200 decode: state_len must be 3, 4 or 5");

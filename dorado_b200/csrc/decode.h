@@ -24,7 +24,8 @@ struct DecodeArgs {
     const b200_qtable* qtable;
     const int32_t* lens;  // optional per-chunk length in SAMPLES (variable chunk sizes); nullptr = every chunk has T blocks
     int stride;           // samples per block (only read with lens)
-    long long* dbg;  // optional clock64 timeline of chunk 0 (B200_DEBUG_BEAM_TIMELINE, test hook only); nullptr in production  // device copy of b200_qtable_build(q_scale, q_shift) (include/b200_crf_math.h)
+    int runners;          // batches in flight on the device (Model::num_runners_hint; < 1 means 1): sizes the state_len 3 grid
+    long long* dbg;  // optional clock64 timeline of chunk 0, state_len 4 and 5 (B200_DEBUG_BEAM_TIMELINE, test hook only); nullptr in production
     // scratch
     float* bwd;   // decode_scratch_bytes() -> bwd_bytes
     uint2* beam;  //                        -> beam_bytes
@@ -37,6 +38,7 @@ struct DecodeArgs {
 
 size_t decode_max_blocks();  // largest T the traceback kernel's shared-memory plan holds
 size_t decode_scratch_bytes(int N, int T, int state_len, size_t* bwd_bytes, size_t* beam_bytes);
+int decode_launches(int state_len);  // kernels one decode_scores call launches
 struct ProfileSink;
 void decode_scores(const DecodeArgs& args, cudaStream_t stream, ProfileSink* prof = nullptr);
 

@@ -438,6 +438,7 @@ void Runner::run_decode(int n, ProfileSink* prof) {
     a.qtable = m_d_qtable;
     a.lens = m_d_lens;
     a.stride = d.stride;
+    a.runners = m_engine.num_runners();
     a.bwd = m_d_bwd;
     a.beam = m_d_beam;
     // output rows are packed for the n chunks actually called
@@ -446,7 +447,7 @@ void Runner::run_decode(int n, ProfileSink* prof) {
     a.qstring = reinterpret_cast<char*>(m_d_out + (size_t)2 * m_N * m_T_out);
     a.n_bases = reinterpret_cast<int32_t*>(m_d_out + nb_offset(m_N, m_T_out));
     decode_scores(a, m_stream, prof);
-    m_engine.gpu_launches += 3;
+    m_engine.gpu_launches += decode_launches(d.state_len);
 }
 
 // Deterministic pseudo-random fp16 signal in [-2, 2) for the batch-size benchmark (an LCG: no <random> state to share).
@@ -749,6 +750,7 @@ void decode_host_scores(int device, const uint16_t* scores, int N, int T, int C,
         B200_CUDA(cudaMemcpyAsync(d_tb, &tb, sizeof(tb), cudaMemcpyHostToDevice, s));
         long long* d_dbg = nullptr;
         if (std::getenv("B200_DEBUG_BEAM_TIMELINE")) {  // test hook only: clock64 stamps of chunk 0, blocks 100..107
+            if (state_len == 3) throw std::invalid_argument("B200_DEBUG_BEAM_TIMELINE: the state_len 3 decode has no timeline");
             B200_CUDA(cudaMalloc(&d_dbg, 128 * sizeof(long long)));
             B200_CUDA(cudaMemsetAsync(d_dbg, 0, 128 * sizeof(long long), s));
             a.dbg = d_dbg;
