@@ -44,7 +44,7 @@ LstmLayerWeights upload_lstm_layer(int C, const float* w_ih, const float* w_hh, 
 void free_lstm_layer(LstmLayerWeights& w);
 
 struct LstmStackDesc {
-    int C = 0;                   // lstm_size: 96, 192, 384, 768 or 1024
+    int C = 0;                   // lstm_size: 96, 128, 192, 256, 384, 768 or 1024
     int T = 0;                   // steps
     int Np = 0;                  // padded batch: a multiple of 16 (lstm_size 96) or 32
     int stride = 1;              // samples per step, for the chunk lengths of set_chunk_lengths
@@ -58,7 +58,7 @@ struct LstmStackDesc {
 // counters and the error word of the grid recurrence
 size_t lstm_stack_workspace_bytes(int C, int num_layers, int T, int Np);
 
-// Every layer is lstm_layer_kernel (lstm_size 96), or the x-projection GEMM followed by lstm_rec_kernel (192, 384) or by
+// Every layer is lstm_layer_kernel (lstm_size 96), or the x-projection GEMM followed by lstm_rec_kernel (128 - 384) or by
 // one or more cooperative launches of lstm_grid_rec_kernel (768, 1024).  Built once per batch shape; reads
 // B200_DEBUG_LSTM_LAYERS, B200_CLUSTER_CHUNKS, B200_GRID_CHUNKS and B200_GRID_GROUPS then.
 class LstmStack {
@@ -70,7 +70,7 @@ public:
     // Enqueues the layers; false if B200_DEBUG_LSTM_LAYERS stopped the stack early (the sequence buffer then holds the
     // output of that many layers)
     bool run(cudaStream_t stream, ProfileSink* prof);
-    // Variable chunk sizes: device array of per-chunk lengths in samples (lstm_size 192 and up)
+    // Variable chunk sizes: device array of per-chunk lengths in samples (lstm_size 128 and up)
     void set_chunk_lengths(const int32_t* d_lens) { m_lens = d_lens; }
     // After the stream has drained: throws if a group of the grid recurrence timed out at its step barrier
     void check_errors();

@@ -5,7 +5,8 @@
 //                                                                                         mma.sync; v5 shapes), conv12_kernel (FMA pipe)
 //   ConvStack layer 3      host_linear "cutlass conv"        dorado/nn/ConvStack.cpp:236-275  -> gemm.cu
 //   LSTMStack              host_cutlass_lstm/host_small_lstm dorado/nn/LSTMStack.cpp:127-238 -> lstm_layer_kernel (lstm_size
-//                                                                                         96), gx GEMM + lstm_rec_kernel (192, 384),
+//                                                                                         96), gx GEMM + lstm_rec_kernel (128, 192,
+//                                                                                         256, 384),
 //                                                                                         gx GEMM + lstm_grid_rec_kernel (768, 1024)
 //   LinearCRF              host_linear                       dorado/nn/CRFModules.cpp:49-122   -> gemm.cu
 // Semantics are those of the CPU modules (ConvStack.cpp:146-163, LSTMStack.cpp:29-41, CRFModules.cpp:24-34).
@@ -506,7 +507,7 @@ __global__ void __launch_bounds__(FL_THREADS, 1) lstm_layer_kernel(const LstmLay
 }
 
 // ------------------------------------------------------------------------------------------------
-// LSTM layer = hoisted x-projection + recurrence (lstm_size 192 and 384).
+// LSTM layer = hoisted x-projection + recurrence (lstm_size 128, 192, 256 and 384).
 //
 // The x_t half of the gate pre-activations does not depend on the recurrence, so it is one large wgmma GEMM per layer
 // (gemm.cu) that writes gx[t][chunk][4C] (fp16, b_ih + b_hh included, PyTorch gate order i | f | g | o).
@@ -522,7 +523,8 @@ __global__ void __launch_bounds__(FL_THREADS, 1) lstm_layer_kernel(const LstmLay
 // mma.sync on register-resident weights keeps that chain short, where wgmma would add its asynchronous hand-offs and a
 // 64-row granularity to every step.  h is double-buffered, so one cluster barrier per step orders both the all-gather of
 // h_t before the MMAs of step t+1 and the reads of h_{t-1} before its buffer is overwritten at step t+1.
-// C = 192 and 384 split over clusters of 4 and 8 CTAs.
+// C = 128 and 192 split over clusters of 4 CTAs, 256 and 384 over clusters of 8 (32 or 48 hidden units per CTA, 256 or 384
+// threads).
 // ------------------------------------------------------------------------------------------------
 
 // CTAs per cluster for a hidden size: the CTA's W_hh rows (4 C / CL x C fp16) must fit its registers
@@ -885,7 +887,9 @@ static void launch_rec_c(const LstmRecParams& rp, int un, int ctas, cudaStream_t
 // Launches lstm_rec_kernel<C, cluster, nb> over `ctas` CTAs; throws Unsupported for a size without an instantiation
 void launch_lstm_rec(int C, int nb, int ctas, const LstmRecParams& p, cudaStream_t stream) {
     switch (C) {
+        case 128: launch_rec_c<128>(p, nb, ctas, stream); break;
         case 192: launch_rec_c<192>(p, nb, ctas, stream); break;
+        case 256: launch_rec_c<256>(p, nb, ctas, stream); break;
         case 384: launch_rec_c<384>(p, nb, ctas, stream); break;
         default: throw Unsupported("no LSTM recurrence instantiation for this lstm_size");
     }
@@ -1199,7 +1203,7 @@ private:
     int pad3() const { return desc.convs[2].winlen / 2; }
     int t_pad(int T_in) const { return T_in + 2 * pad3() + 8; }
     // lstm_size 96 keeps the reference's fixed-size contract (batch a multiple of 16, no variable chunk sizes); the larger
-    // sizes take batches in multiples of 32 and variable chunk sizes
+    // sizes, 128 included, take batches in multiples of 32 and variable chunk sizes
     bool large() const { return desc.lstm_size > 96; }
     int n_pad(int N) const { return large() ? (N + 31) / 32 * 32 : (N + 15) / 16 * 16; }
 };
@@ -1213,9 +1217,9 @@ LstmModel::LstmModel(const b200_model_desc& d, const b200_tensor* tensors, int n
     }
     const int C = d.lstm_size;
     if (C != c3.size) throw std::invalid_argument("last convolution size != lstm_size");
-    if (C != 96 && C != 192 && C != 384 && C != 768 && C != 1024) {
+    if (C != 96 && C != 128 && C != 192 && C != 256 && C != 384 && C != 768 && C != 1024) {
         // kernels are instantiated for the sizes of the reference's model zoo this engine covers
-        throw Unsupported("lstm_size " + std::to_string(C) + " is not supported (96, 192, 384, 768 and 1024 are)");
+        throw Unsupported("lstm_size " + std::to_string(C) + " is not supported (96, 128, 192, 256, 384, 768 and 1024 are)");
     }
 
     if (d.lstm_layers < 1 || d.lstm_layers > 8) throw std::invalid_argument("bad lstm_layers");

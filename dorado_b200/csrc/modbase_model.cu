@@ -229,8 +229,8 @@ ModBaseEngine::ModBaseEngine(const b200_modbase_desc& d, const b200_tensor* tens
         throw Unsupported("modbase: convolution shapes outside what the kernels implement");
     }
     const int C = d.lstm_size;
-    if (C != 192 && C != 384 && C != 768 && C != 1024) {
-        throw Unsupported("modbase: lstm_size " + std::to_string(C) + " is not supported (192, 384, 768 and 1024 are)");
+    if (C != 128 && C != 192 && C != 256 && C != 384 && C != 768 && C != 1024) {
+        throw Unsupported("modbase: lstm_size " + std::to_string(C) + " is not supported (128, 192, 256, 384, 768 and 1024 are)");
     }
     if (seq_conv1_smem(q1.insize, q1.winlen) > (size_t)SQ_MAX_SMEM) throw Unsupported("modbase: seq_conv1 too wide for shared memory");
     if (d.num_out > HEAD_MAX_OUT || d.upsample_scale < 0 || d.upsample_scale * d.num_out > HEAD_MAX_UP) {

@@ -167,8 +167,10 @@ B200_API int b200_runner_accept_chunk_f32(b200_runner* runner, int32_t chunk_idx
 /* Variable chunk sizes (SURVEY.md 8f row 1; CudaCaller::variable_chunk_sizes, api/runner_creation.cpp:24-42,
  * CudaModelRunner::accept_chunk CudaModelRunner.cpp:21-31, nn/AuxiliaryData.cpp:19-124, CUDADecoder.cpp:35-62,126-147):
  * chunks of different lengths share a batch, so a read's tail is not repeat-padded to chunk_size and the work for it shrinks.
- * b200_runner_variable_chunk_sizes() is 1 for the models the mode exists for (plain LSTM models of lstm_size 192, 384,
- * 768 and 1024; not FLSTM); b200_runner_accept_chunk_var_f16 takes `len` samples, a positive multiple of the model stride and
+ * b200_runner_variable_chunk_sizes() is 1 for the models the mode exists for (plain LSTM models of lstm_size 128, 192, 256,
+ * 384, 768 and 1024; not FLSTM).  The reference runs the mode only for multiples of 128 above 128
+ * (check_variable_chunk_sizes_supported, api/runner_creation.cpp:28-31), so here 128 and 192 accept it where the reference
+ * would call fixed-size chunks.  b200_runner_accept_chunk_var_f16 takes `len` samples, a positive multiple of the model stride and
  * <= chunk_size (BasecallerNode wraps a read's tail round to the next stride multiple, BasecallerNode.cpp:408-417).  The
  * reference packs the batch as one [1, C, sum T] row with an (offset, length) table; here every chunk keeps its slot and the
  * kernels read the length table: the convolutions see zero padding at the chunk's own end, the recurrence holds a zero
@@ -381,7 +383,7 @@ typedef struct b200_modbase_desc {
     b200_conv_desc sig_convs[3];   /* ModulesParams::signal_convs: 1 -> c1 (<= 16) -> 16 -> C_sig */
     b200_conv_desc seq_convs[2];   /* ModulesParams::sequence_convs: kmer_len * 4 -> 16 -> C_seq */
     b200_conv_desc merge_conv;     /* C_sig + C_seq -> lstm_size */
-    int32_t lstm_size;             /* both LSTM layers: 192 or 384 (cluster kernel), 768 or 1024 (grid kernel) */
+    int32_t lstm_size;             /* both LSTM layers: 128, 192, 256 or 384 (cluster kernel), 768 or 1024 (grid kernel) */
     int32_t num_out;               /* linear out_features */
     int32_t upsample_scale;        /* LinearUpsample scale_factor, 0 = no upsample */
     int32_t kmer_len;

@@ -1,14 +1,14 @@
 #!/usr/bin/env python
-"""Throughput of the lstm_size 768 / 1024 models (lstm_grid_rec_kernel) on one GPU.
+"""Throughput of the lstm_size 128 / 256 models (lstm_rec_kernel) and 768 / 1024 models (lstm_grid_rec_kernel) on one GPU.
 
-usage: python tools/bench_wide_lstm.py --model lstm768|lstm1024 [--batch 512] [--chunksize 10000] [--runners 2]
-       [--steps 50] [--warmup 3]
+usage: python tools/bench_wide_lstm.py --model lstm128|lstm256|lstm768|lstm1024 [--batch 512] [--chunksize 10000]
+       [--runners 2] [--steps 50] [--warmup 3]
 
 Device-resident steps as bench.py times them (step i on runner i % R, each runner on its own stream), then one profiled
 forward + decode with an event after every launch.  Prints one JSON line: samples/s, the per-kernel times of the profiled
-pass, the recurrence time per layer and per step, and the recurrence's W_hh FLOP over its time against the dense fp16 peak
-of the H100 SXM data sheet (989 TFLOP/s, a 700 W card; not a measured peak).  FLOP per sample come from the config's
-shapes: per output step 16 C^2 per LSTM layer, conv3 and the CRF linear.
+pass, the x-projection GEMM and recurrence times per layer, the recurrence time per step, and the recurrence's W_hh FLOP
+over its time against the dense fp16 peak of the H100 SXM data sheet (989 TFLOP/s, a 700 W card; not a measured peak).
+FLOP per sample come from the config's shapes: per output step 16 C^2 per LSTM layer, conv3 and the CRF linear.
 """
 import argparse
 import json
@@ -25,12 +25,13 @@ PEAK_TFLOPS = 989.0
 
 
 def main():
-    from test_wide_lstm_cpu import model_dir
+    import test_lstm128_256_cpu
+    import test_wide_lstm_cpu
     from dorado_b200.config import load_model_config
     from dorado_b200.runner import B200Caller, B200ModelRunner
     from dorado_b200.weights import synthetic_weights
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", required=True, choices=["lstm768", "lstm1024"])
+    ap.add_argument("--model", required=True, choices=["lstm128", "lstm256", "lstm768", "lstm1024"])
     ap.add_argument("--batch", type=int, default=512)
     ap.add_argument("--chunksize", type=int, default=10000)
     ap.add_argument("--runners", type=int, default=2)
@@ -38,7 +39,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     args = ap.parse_args()
 
-    cfg = load_model_config(model_dir(args.model))
+    cluster = args.model in test_lstm128_256_cpu.MODELS   # lstm_rec_kernel, else lstm_grid_rec_kernel
+    cfg = load_model_config((test_lstm128_256_cpu if cluster else test_wide_lstm_cpu).model_dir(args.model))
     C, c3 = cfg.lstm_size, cfg.convs[2]
     flop_per_sample = (cfg.lstm_layers * 16.0 * C * C + 2.0 * c3.winlen * c3.insize * C + 2.0 * C * cfg.outsize) / cfg.stride
     N, R = args.batch, max(1, args.runners)
@@ -59,7 +61,8 @@ def main():
         k, tot = prof.get(name, (0, 0.0))
         prof[name] = (k + 1, tot + t)
     plan = runners[0].plan_info()
-    launches, rec_ms = prof["lstm_grid_rec"]
+    mark, key = ("lstm_rec", "lstm_rec.ctas") if cluster else ("lstm_grid_rec", "lstm_grid.ctas")
+    launches, rec_ms = prof[mark]
     layer_ms = rec_ms / cfg.lstm_layers
     rec_tflops = 8.0 * C * C * T_out * N * cfg.lstm_layers / (rec_ms * 1e-3) / 1e12
     out = {"model": args.model, "lstm_size": C, "batch": N, "chunk_samples": T, "runners": R, "steps": args.steps,
@@ -67,10 +70,11 @@ def main():
            "flop_per_sample": flop_per_sample, "forward_tflops_per_s": flop_per_sample * value / 1e12,
            "plan": plan,
            "kernels_ms": {k: {"launches": n, "ms": round(t, 4)} for k, (n, t) in prof.items()},
-           "lstm_grid_rec": {"ms_per_layer": layer_ms, "ms_per_launch": rec_ms / launches,
-                             "us_per_step": rec_ms / launches / T_out * 1e3, "tflops": rec_tflops,
-                             "frac_of_peak": rec_tflops / PEAK_TFLOPS,
-                             "frac_of_sms_used": rec_tflops / PEAK_TFLOPS * 132 / plan["lstm_grid.ctas"]}}
+           "gx_gemm_ms_per_layer": prof["lstm_gx_gemm"][1] / cfg.lstm_layers,
+           mark: {"ms_per_layer": layer_ms, "ms_per_launch": rec_ms / launches,
+                  "us_per_step": rec_ms / launches / T_out * 1e3, "tflops": rec_tflops,
+                  "frac_of_peak": rec_tflops / PEAK_TFLOPS,
+                  "frac_of_sms_used": rec_tflops / PEAK_TFLOPS * 132 / min(132, plan[key])}}
     print(json.dumps(out))
     for r in runners:
         r.close()
