@@ -374,6 +374,14 @@ int b200_test_gemm(int32_t device, const uint16_t* a, const uint16_t* b, const f
     });
 }
 
+int b200_test_attention(int32_t device, const uint16_t* qkv, int32_t N, int32_t T, int32_t H, int32_t win_upper,
+                        int32_t win_lower, uint16_t* out) {
+    return guarded([&] {
+        if (!qkv || !out) throw std::invalid_argument("b200_test_attention: null argument");
+        b200::test_attention_host(device, qkv, N, T, H, win_upper, win_lower, out);
+    });
+}
+
 }  // extern "C"
 
 // ---- modified-base models -------------------------------------------------------------------------------------------

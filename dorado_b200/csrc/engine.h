@@ -338,6 +338,7 @@ void decode_host_scores(int device, const uint16_t* scores, int N, int T, int C,
                         int32_t* n_bases);
 void test_gemm_host(int device, const uint16_t* a, const uint16_t* b, const float* bias, int M, int N, int K,
                     int activation, uint16_t* c);
+void test_attention_host(int device, const uint16_t* qkv, int N, int T, int H, int win_upper, int win_lower, uint16_t* out);
 
 // batch-size selection (CudaCaller::determine_batch_dims)
 size_t runner_device_bytes(Engine& engine, int batch_size, int chunk_size);

@@ -91,7 +91,7 @@ EXPORTS = [
     "b200_runner_set_decoder_options", "b200_runner_batch_size", "b200_runner_chunk_size", "b200_runner_out_len",
     "b200_runner_accept_chunk_f16", "b200_runner_accept_chunk_f32", "b200_runner_input", "b200_runner_call_chunks",
     "b200_runner_upload", "b200_runner_step_device", "b200_runners_step_device", "b200_runner_forward_scores", "b200_runner_profile", "b200_runner_plan_info", "b200_runner_debug_read_workspace", "b200_decode_scores",
-    "b200_test_gemm", "b200_generate_chunks", "b200_stitch_chunks", "b200_runner_accept_raw_chunk",
+    "b200_test_gemm", "b200_test_attention", "b200_generate_chunks", "b200_stitch_chunks", "b200_runner_accept_raw_chunk",
     "b200_runner_debug_read_input", "b200_engine_runner_bytes", "b200_engine_benchmark_batch_sizes",
     "b200_select_batch_size", "b200_generate_variable_chunks", "b200_engine_terminate", "b200_engine_restart",
     "b200_engine_set_low_latency", "b200_engine_is_low_latency", "b200_engine_batch_timeouts_ms",
@@ -172,6 +172,7 @@ def load_library() -> C.CDLL:
     lib.b200_runner_plan_info.argtypes = [vp, C.c_char_p, C.c_uint64]
     lib.b200_runner_debug_read_workspace.argtypes = [vp, C.c_uint64, C.c_uint64, vp]
     lib.b200_test_gemm.argtypes = [i32, vp, vp, vp, i32, i32, i32, i32, vp]
+    lib.b200_test_attention.argtypes = [i32, vp, i32, i32, i32, i32, i32, vp]
     u64 = C.c_uint64
     lib.b200_generate_chunks.argtypes = [u64, u64, u64, u64, C.POINTER(u64), u64, C.POINTER(u64)]
     lib.b200_generate_variable_chunks.argtypes = [u64, u64, u64, u64, C.POINTER(u64), u64, C.POINTER(u64)]
@@ -273,3 +274,14 @@ def test_gemm(a: np.ndarray, b: np.ndarray, bias: np.ndarray | None, activation:
         bias_p = bias.ctypes.data
     check(lib.b200_test_gemm(device, a.ctypes.data, b.ctypes.data, bias_p, M, N, K, activation, c.ctypes.data))
     return c
+
+
+def test_attention(qkv: np.ndarray, win_upper: int, win_lower: int, device: int = 0):
+    """The model's attention kernel on host data: qkv [N, T, 3, H, 64] fp16 -> out [N, T, H * 64] fp16."""
+    lib = load_library()
+    qkv = np.ascontiguousarray(qkv, np.float16)
+    N, T, three, H, D = qkv.shape
+    assert three == 3 and D == 64
+    out = np.empty((N, T, H * 64), np.float16)
+    check(lib.b200_test_attention(device, qkv.ctypes.data, N, T, H, win_upper, win_lower, out.ctypes.data))
+    return out

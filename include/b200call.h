@@ -59,7 +59,10 @@ typedef struct b200_model_desc {
     int32_t linear_bias;  /* config.bias */
     int32_t out_features; /* 0 = no linear decomposition */
     float crf_scale;      /* 5.0 => tanh(x)*5 on the last linear (pre-v4.x models) */
-    /* transformer models (dorado/nn/TxModules.cpp, dorado/basecall/model/TxModel.cpp) */
+    /* transformer models (dorado/nn/TxModules.cpp, dorado/basecall/model/TxModel.cpp).  Accepted shapes: d_model == 64 * nhead
+     * (head dimension 64), d_model a multiple of 128 and at most 1536, dim_feedforward a multiple of 64, attention windows
+     * 0 <= attn_window_upper, attn_window_lower <= 256 -- e.g. sup (512, 8 heads, (127, 128), 2048) and the 1536-wide
+     * encoder (24 heads, (255, 256), 6144).  Anything else returns B200_ERR_UNSUPPORTED from b200_engine_create. */
     int32_t d_model, nhead, dim_feedforward, depth;
     int32_t attn_window_upper, attn_window_lower;
     int32_t upsample_scale, max_seq_len;
@@ -437,6 +440,11 @@ B200_API int b200_modbase_runner_debug_read_workspace(b200_modbase_runner* runne
 B200_API int b200_test_gemm(int32_t device, const uint16_t* a /* [M,K] fp16 */, const uint16_t* b /* [N,K] fp16 */,
                             const float* bias /* [N] or NULL */, int32_t M, int32_t N, int32_t K, int32_t activation,
                             uint16_t* c /* [M,N] fp16 */);
+/* The transformer's sliding-window attention kernel, launched exactly as the model launches it: qkv of N chunks of T tokens
+ * (q and k already rotated), query i of a chunk attends keys j with -win_upper <= j - i <= win_lower, softmax scale 1/8.
+ * Windows outside [0, 256] return B200_ERR_UNSUPPORTED. */
+B200_API int b200_test_attention(int32_t device, const uint16_t* qkv /* [N*T][3][H][64] fp16 */, int32_t N, int32_t T,
+                                 int32_t H, int32_t win_upper, int32_t win_lower, uint16_t* out /* [N*T][H*64] fp16 */);
 
 #ifdef __cplusplus
 }
