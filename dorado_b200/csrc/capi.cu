@@ -374,6 +374,28 @@ int b200_test_gemm(int32_t device, const uint16_t* a, const uint16_t* b, const f
     });
 }
 
+int b200_test_gemm_fp8(int32_t device, const uint8_t* a, const uint8_t* b, int32_t M, int32_t N, int32_t K, int32_t activation,
+                       const uint16_t* residual, float alpha, void* c) {
+    return guarded([&] {
+        if (!a || !b || !c) throw std::invalid_argument("b200_test_gemm_fp8: null argument");
+        b200::test_gemm_fp8_host(device, a, b, M, N, K, activation, residual, alpha, c);
+    });
+}
+
+int b200_test_to_e4m3(const uint16_t* f16, int64_t n, uint8_t* out) {
+    return guarded([&] {
+        if (n < 0 || (n && (!f16 || !out))) throw std::invalid_argument("b200_test_to_e4m3: bad argument");
+        for (int64_t i = 0; i < n; ++i) out[i] = b200::e4m3_from_f16_bits(f16[i]);
+    });
+}
+
+int b200_test_remove_bits(const uint16_t* f16, int64_t n, int32_t bits, uint16_t* out) {
+    return guarded([&] {
+        if (n < 0 || (n && (!f16 || !out)) || bits < 0 || bits > 10) throw std::invalid_argument("b200_test_remove_bits: bad argument");
+        for (int64_t i = 0; i < n; ++i) out[i] = b200::remove_bits_f16(f16[i], bits);
+    });
+}
+
 int b200_test_attention(int32_t device, const uint16_t* qkv, int32_t N, int32_t T, int32_t H, int32_t win_upper,
                         int32_t win_lower, uint16_t* out) {
     return guarded([&] {

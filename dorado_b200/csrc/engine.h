@@ -339,6 +339,15 @@ void decode_host_scores(int device, const uint16_t* scores, int N, int T, int C,
 void test_gemm_host(int device, const uint16_t* a, const uint16_t* b, const float* bias, int M, int N, int K,
                     int activation, uint16_t* c);
 void test_attention_host(int device, const uint16_t* qkv, int N, int T, int H, int win_upper, int win_lower, uint16_t* out);
+void test_gemm_fp8_host(int device, const uint8_t* a, const uint8_t* b, int M, int N, int K, int activation,
+                        const uint16_t* residual, float alpha, void* c);
+
+// Host rounding of the fp8_ffn weights (tx_model.cu): fp16 bits of a float (round to nearest even), the reference's
+// remove_bits on fp16 bits, fp16(v) with remove_bits as float, and torch's float8_e4m3fn cast of an fp16 value.
+uint16_t f16_bits(float v);
+uint16_t remove_bits_f16(uint16_t b, int bits);
+std::vector<float> fp16_remove_bits(const float* v, size_t n, int bits);
+uint8_t e4m3_from_f16_bits(uint16_t b);
 
 // batch-size selection (CudaCaller::determine_batch_dims)
 size_t runner_device_bytes(Engine& engine, int batch_size, int chunk_size);

@@ -8,6 +8,8 @@
 // A and W tiles, 128-byte swizzle, a STAGES-deep mbarrier ring that runs across tiles); warpgroups 1 and 2 own rows 0-63 and
 // 64-127 of the tile: they issue wgmma m64n32k16 straight from the swizzled stages, keep the fp32 accumulator in registers
 // and run the epilogue (bias / activation / residual / rotary / SwiGLU -> fp16 -> global) from the accumulator fragments.
+// E4M3 form (template FP8, the transformer's fc1 / fc2 in the fp8_ffn precision): the same ring, tiles and epilogues with
+// 128 E4M3 per 128-byte K row instead of 64 fp16, wgmma m64n32k32.e4m3 and the SwiGLU output cast to E4M3.
 // A is addressed through a 3-D tensor map (k, row, batch) so that overlapping-row views work: the last conv of the LSTM
 // models reads its im2col rows straight from the NTC activation buffer with row stride = stride * C_in (the reference's
 // "cutlass_conv" trick, ConvStack.cpp:236-275).
@@ -25,7 +27,8 @@ namespace b200 {
 namespace {
 
 constexpr int BM = 128;
-constexpr int BK = 64;
+constexpr int BK = 64;              // fp16 per K block: one 128-byte swizzle row (128 E4M3 in the fp8 form)
+constexpr int BK8 = 128;
 constexpr int BN_MAX = 128;
 constexpr int STAGES = 5;          // TMA -> wgmma ring depth: 5 x 32 KB of the 227 KB
 constexpr int GEMM_PARTS = 4;      // RMSNorm partial sums per row and column tile (GemmDesc::out_ss): one per 32-column chunk
@@ -81,28 +84,33 @@ __device__ __forceinline__ float act_apply(float v) {
     else return v;
 }
 
-// One K block (64) of a warpgroup's 64 x 32 NCH tile: 32 rows of W are 4 KB further on, 16 fp16 along K are +2 in the
-// (addr >> 4) field of a descriptor.
-template <int NCH>
+// One K block (128 bytes: 64 fp16 or 128 E4M3) of a warpgroup's 64 x 32 NCH tile: 32 rows of W are 4 KB further on,
+// 32 bytes along K (16 fp16, 32 E4M3: one wgmma) are +2 in the (addr >> 4) field of a descriptor.
+template <int NCH, bool FP8>
 __device__ __forceinline__ void wgmma_k_block(float (&acc)[BN_MAX / 32][16], uint64_t adesc, uint64_t bdesc, bool accumulate) {
 #pragma unroll
-    for (int k = 0; k < BK / 16; ++k) {
+    for (int k = 0; k < 4; ++k) {
 #pragma unroll
         for (int c = 0; c < NCH; ++c) {
-            tc::wgmma_m64n32k16(acc[c], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(c * 256 + 2 * k), accumulate || k != 0);
+            if constexpr (FP8) {
+                tc::wgmma_m64n32k32_e4m3(acc[c], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(c * 256 + 2 * k), accumulate || k != 0);
+            } else {
+                tc::wgmma_m64n32k16(acc[c], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(c * 256 + 2 * k), accumulate || k != 0);
+            }
         }
     }
 }
 
-template <int ACT>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a,
-                                                                         const __grid_constant__ CUtensorMap tma_w,
-                                                                         const GemmKernelParams p) {
+template <int ACT, bool FP8>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a,
+                                                                     const __grid_constant__ CUtensorMap tma_w,
+                                                                     const GemmKernelParams p) {
+    constexpr int KB = FP8 ? BK8 : BK;   // K elements per block
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // realign by an integer offset from the __shared__ symbol so the compiler keeps the shared address space
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
-    const uint32_t a_bytes = BM * BK * 2;
-    const uint32_t w_bytes = (uint32_t)p.bn * BK * 2;   // a multiple of 4 KB: every stage stays 1024-byte aligned
+    const uint32_t a_bytes = BM * 128;
+    const uint32_t w_bytes = (uint32_t)p.bn * 128;   // a multiple of 4 KB: every stage stays 1024-byte aligned
     const uint32_t stage_bytes = a_bytes + w_bytes;
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * stage_bytes);
     uint64_t* empty = full + STAGES;
@@ -132,8 +140,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_wgmma_kernel(const _
                     tc::mbar_wait_silent(&empty[s], ph ^ 1);
                     tc::mbar_arrive_expect_tx(&full[s], stage_bytes);
                     uint8_t* st = smem + s * stage_bytes;
-                    tc::tma_load_3d(st, &tma_a, &full[s], kb * BK, r0, batch);
-                    tc::tma_load_2d(st + a_bytes, &tma_w, &full[s], kb * BK, nt * p.bn);
+                    tc::tma_load_3d(st, &tma_a, &full[s], kb * KB, r0, batch);
+                    tc::tma_load_2d(st + a_bytes, &tma_w, &full[s], kb * KB, nt * p.bn);
                     if (++s == STAGES) {
                         s = 0;
                         ph ^= 1;
@@ -162,10 +170,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_wgmma_kernel(const _
             const uint64_t bdesc = tc::wgmma_desc_sw128(st + a_bytes);
             tc::wgmma_fence();
             switch (nch) {   // the chunk count as a constant: no predicated wgmma, no registers ptxas must fence
-                case 1: wgmma_k_block<1>(acc, adesc, bdesc, kb != 0); break;
-                case 2: wgmma_k_block<2>(acc, adesc, bdesc, kb != 0); break;
-                case 3: wgmma_k_block<3>(acc, adesc, bdesc, kb != 0); break;
-                default: wgmma_k_block<4>(acc, adesc, bdesc, kb != 0); break;
+                case 1: wgmma_k_block<1, FP8>(acc, adesc, bdesc, kb != 0); break;
+                case 2: wgmma_k_block<2, FP8>(acc, adesc, bdesc, kb != 0); break;
+                case 3: wgmma_k_block<3, FP8>(acc, adesc, bdesc, kb != 0); break;
+                default: wgmma_k_block<4, FP8>(acc, adesc, bdesc, kb != 0); break;
             }
             tc::wgmma_commit();
             // one group stays in flight: the previous K block's group has completed, so its stage goes back to the producer
@@ -262,7 +270,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_f16_wgmma_kernel(const _
                         float v1 = acc[c][4 * j + 2 * h + 1] * r_a[h] + b2.y + row_bias[h];
                         if constexpr (ACT == GEMM_ACT_SWIGLU) {
                             // columns (2i, 2i + 1) = (y, gate) -> output column i
-                            p.out[off[h] + nc / 2] = __float2half_rn(v0 * swish_fast(v1));
+                            if constexpr (FP8) {
+                                reinterpret_cast<uint8_t*>(p.out)[off[h] + nc / 2] = (uint8_t)tc::cvt_e4m3x2(v0 * swish_fast(v1), 0.0f);
+                            } else {
+                                p.out[off[h] + nc / 2] = __float2half_rn(v0 * swish_fast(v1));
+                            }
                         } else {
                             if (p.residual) {
                                 const float2 f = __half22float2(
@@ -316,10 +328,11 @@ EncodeFn get_encode_fn() {
 }
 
 CUtensorMap encode(const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-                   const cuuint32_t* box, CUtensorMapSwizzle swz) {
+                   const cuuint32_t* box, CUtensorMapSwizzle swz, uint32_t elem_bytes) {
     CUtensorMap m;
     cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-    const CUresult r = get_encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(base), dims,
+    const CUtensorMapDataType dt = elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    const CUresult r = get_encode_fn()(&m, dt, (cuuint32_t)rank, const_cast<void*>(base), dims,
                                        strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
                                        CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
@@ -331,25 +344,25 @@ CUtensorMap encode(const void* base, int rank, const cuuint64_t* dims, const cuu
 }  // namespace
 
 CUtensorMap make_tmap_2d(const void* base, uint64_t inner, uint64_t outer, uint64_t outer_stride_bytes, uint32_t box_inner,
-                         uint32_t box_outer) {
+                         uint32_t box_outer, uint32_t elem_bytes) {
     const cuuint64_t dims[2] = {inner, outer};
     const cuuint64_t strides[1] = {outer_stride_bytes};
     const cuuint32_t box[2] = {box_inner, box_outer};
-    const CUtensorMapSwizzle swz = box_inner * 2 == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                                   : box_inner * 2 == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                                                         : CU_TENSOR_MAP_SWIZZLE_NONE;
-    return encode(base, 2, dims, strides, box, swz);
+    const CUtensorMapSwizzle swz = box_inner * elem_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
+                                   : box_inner * elem_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                                                  : CU_TENSOR_MAP_SWIZZLE_NONE;
+    return encode(base, 2, dims, strides, box, swz, elem_bytes);
 }
 
 CUtensorMap make_tmap_3d(const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t s1_bytes, uint64_t s2_bytes,
-                         uint32_t b0, uint32_t b1, uint32_t b2) {
+                         uint32_t b0, uint32_t b1, uint32_t b2, uint32_t elem_bytes) {
     const cuuint64_t dims[3] = {d0, d1, d2};
     const cuuint64_t strides[2] = {s1_bytes, s2_bytes};
     const cuuint32_t box[3] = {b0, b1, b2};
-    const CUtensorMapSwizzle swz = b0 * 2 == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                                   : b0 * 2 == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                                                  : CU_TENSOR_MAP_SWIZZLE_NONE;
-    return encode(base, 3, dims, strides, box, swz);
+    const CUtensorMapSwizzle swz = b0 * elem_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
+                                   : b0 * elem_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                                           : CU_TENSOR_MAP_SWIZZLE_NONE;
+    return encode(base, 3, dims, strides, box, swz, elem_bytes);
 }
 
 static int pick_bn(int N) {
@@ -367,10 +380,17 @@ int gemm_out_ss_parts(int N) {
 }
 
 GemmPlan make_gemm_plan(const GemmDesc& d) {
-    if (d.K % BK != 0 || d.K <= 0) throw std::invalid_argument("gemm: K must be a positive multiple of 64");
+    const int kb = d.fp8 ? BK8 : BK;
+    const int eb = d.fp8 ? 1 : 2;   // bytes per A / W element
+    if (d.K % kb != 0 || d.K <= 0) {
+        throw std::invalid_argument(d.fp8 ? "gemm: E4M3 K must be a positive multiple of 128" : "gemm: K must be a positive multiple of 64");
+    }
+    if (d.fp8 && (d.act != GEMM_ACT_NONE && d.act != GEMM_ACT_SWIGLU)) {
+        throw std::invalid_argument("gemm: E4M3 operands take the plain and SwiGLU epilogues only");
+    }
     if (d.N % 32 != 0) throw std::invalid_argument("gemm: N must be a multiple of 32");
     if (d.batches < 1 || d.rows_per_batch < 1) throw std::invalid_argument("gemm: empty A");
-    if ((d.a_row_stride * 2) % 16 != 0 || (d.a_batch_stride * 2) % 16 != 0) {
+    if ((d.a_row_stride * eb) % 16 != 0 || (d.a_batch_stride * eb) % 16 != 0) {
         throw std::invalid_argument("gemm: A strides must be multiples of 16 bytes");
     }
     GemmPlan p{};
@@ -399,20 +419,20 @@ GemmPlan make_gemm_plan(const GemmDesc& d) {
         throw std::invalid_argument("gemm: rows and output blocking must fit 32-bit index arithmetic");
     }
     p.grid = dim3((unsigned)(p.tiles_per_batch * d.batches), (unsigned)(d.N / p.bn), 1);
-    p.smem = (size_t)STAGES * ((size_t)BM * BK * 2 + (size_t)p.bn * BK * 2) + 256 + 1024;
+    p.smem = (size_t)STAGES * ((size_t)BM * 128 + (size_t)p.bn * 128) + 256 + 1024;
     if (p.smem > 227 * 1024) throw std::logic_error("gemm: shared-memory plan does not fit");
-    const uint64_t batch_stride = d.batches > 1 ? (uint64_t)d.a_batch_stride * 2 : (uint64_t)d.a_row_stride * 2 * d.rows_per_batch;
-    p.tma_a = make_tmap_3d(d.a, (uint64_t)(d.a_inner > 0 ? d.a_inner : d.K), (uint64_t)d.rows_per_batch, (uint64_t)d.batches, (uint64_t)d.a_row_stride * 2,
-                           batch_stride, BK, BM, 1);
-    p.tma_w = make_tmap_2d(d.w, (uint64_t)d.K, (uint64_t)d.N, (uint64_t)d.K * 2, BK, (uint32_t)p.bn);
+    const uint64_t batch_stride = d.batches > 1 ? (uint64_t)d.a_batch_stride * eb : (uint64_t)d.a_row_stride * eb * d.rows_per_batch;
+    p.tma_a = make_tmap_3d(d.a, (uint64_t)(d.a_inner > 0 ? d.a_inner : d.K), (uint64_t)d.rows_per_batch, (uint64_t)d.batches, (uint64_t)d.a_row_stride * eb,
+                           batch_stride, kb, BM, 1, eb);
+    p.tma_w = make_tmap_2d(d.w, (uint64_t)d.K, (uint64_t)d.N, (uint64_t)d.K * eb, kb, (uint32_t)p.bn, eb);
     return p;
 }
 
-template <int ACT>
+template <int ACT, bool FP8 = false>
 static void launch_gemm(int grid, size_t smem, cudaStream_t stream, const CUtensorMap& a, const CUtensorMap& w,
                         const GemmKernelParams& k) {
-    ensure_dynamic_smem(gemm_f16_wgmma_kernel<ACT>, 227 * 1024);
-    gemm_f16_wgmma_kernel<ACT><<<grid, GEMM_THREADS, smem, stream>>>(a, w, k);
+    ensure_dynamic_smem(gemm_wgmma_kernel<ACT, FP8>, 227 * 1024);
+    gemm_wgmma_kernel<ACT, FP8><<<grid, GEMM_THREADS, smem, stream>>>(a, w, k);
 }
 
 void run_gemm(const GemmPlan& p, cudaStream_t stream) {
@@ -420,10 +440,10 @@ void run_gemm(const GemmPlan& p, cudaStream_t stream) {
     k.rows_per_batch = p.d.rows_per_batch;
     k.tiles_per_batch = p.tiles_per_batch;
     k.N = p.d.N;
-    k.num_k_blocks = p.d.K / BK;
+    k.num_k_blocks = p.d.K / (p.d.fp8 ? BK8 : BK);
     k.bn = p.bn;
     k.bias = p.d.bias;
-    k.out = p.d.out;
+    k.out = static_cast<__half*>(p.d.out);
     k.out_m1 = (uint32_t)p.d.out_m1;
     k.out_s0 = p.d.out_s0;
     k.out_s1 = p.d.out_s1;
@@ -450,6 +470,12 @@ void run_gemm(const GemmPlan& p, cudaStream_t stream) {
     k.norm_eps = p.d.norm_eps;
     const int max_ctas = p.d.max_ctas > 0 && p.d.max_ctas < kNumSMs ? p.d.max_ctas : kNumSMs;
     const int grid = k.num_tiles < max_ctas ? k.num_tiles : max_ctas;
+    if (p.d.fp8) {
+        if (p.d.act == GEMM_ACT_SWIGLU) launch_gemm<GEMM_ACT_SWIGLU, true>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
+        else launch_gemm<GEMM_ACT_NONE, true>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
+        B200_CUDA(cudaGetLastError());
+        return;
+    }
     switch (p.d.act) {
         case GEMM_ACT_NONE: launch_gemm<GEMM_ACT_NONE>(grid, p.smem, stream, p.tma_a, p.tma_w, k); break;
         case GEMM_ACT_SWISH: launch_gemm<GEMM_ACT_SWISH>(grid, p.smem, stream, p.tma_a, p.tma_w, k); break;
@@ -501,6 +527,52 @@ void test_gemm_host(int device, const uint16_t* a, const uint16_t* b, const floa
     run_gemm(plan, nullptr);
     B200_CUDA(cudaDeviceSynchronize());
     B200_CUDA(cudaMemcpy(c, d_c, (size_t)M * n_out * 2, cudaMemcpyDeviceToHost));
+}
+
+// E4M3 operands (A [M][K], W [N][K] bytes, K zero-padded to a multiple of 128): the plain epilogue with an optional deepnorm
+// residual (c = A W^T + alpha * residual, fp16) or the SwiGLU epilogue (c = E4M3 [M][N / 2]).
+void test_gemm_fp8_host(int device, const uint8_t* a, const uint8_t* b, int M, int N, int K, int activation,
+                        const uint16_t* residual, float alpha, void* c) {
+    if (M < 1 || N < 1 || K < 1) throw std::invalid_argument("test_gemm_fp8: empty operand");
+    if (activation != GEMM_ACT_NONE && activation != GEMM_ACT_SWIGLU) throw std::invalid_argument("test_gemm_fp8: plain or SwiGLU only");
+    if (residual && activation != GEMM_ACT_NONE) throw std::invalid_argument("test_gemm_fp8: the residual goes with the plain epilogue");
+    require_sm90(device);
+    const int Kp = (K + BK8 - 1) / BK8 * BK8;
+    const bool swiglu = activation == GEMM_ACT_SWIGLU;
+    const int n_out = swiglu ? N / 2 : N;
+    const size_t out_bytes = (size_t)M * n_out * (swiglu ? 1 : 2);
+    Arena arena;
+    arena.reserve((size_t)M * Kp + (size_t)N * Kp + (size_t)M * N * 2 + out_bytes + 4096);
+    auto* d_a = static_cast<uint8_t*>(arena.take((size_t)M * Kp));
+    auto* d_w = static_cast<uint8_t*>(arena.take((size_t)N * Kp));
+    auto* d_res = static_cast<__half*>(arena.take((size_t)M * N * 2));
+    void* d_c = arena.take(out_bytes);
+    B200_CUDA(cudaMemset(d_a, 0, (size_t)M * Kp));
+    B200_CUDA(cudaMemset(d_w, 0, (size_t)N * Kp));
+    B200_CUDA(cudaMemcpy2D(d_a, (size_t)Kp, a, (size_t)K, (size_t)K, M, cudaMemcpyHostToDevice));
+    B200_CUDA(cudaMemcpy2D(d_w, (size_t)Kp, b, (size_t)K, (size_t)K, N, cudaMemcpyHostToDevice));
+    if (residual) B200_CUDA(cudaMemcpy(d_res, residual, (size_t)M * N * 2, cudaMemcpyHostToDevice));
+    GemmDesc d{};
+    d.fp8 = 1;
+    d.a = d_a;
+    d.batches = 1;
+    d.rows_per_batch = M;
+    d.a_row_stride = Kp;
+    d.a_batch_stride = (int64_t)M * Kp;
+    d.w = d_w;
+    d.N = N;
+    d.K = Kp;
+    d.act = activation;
+    d.out = d_c;
+    d.out_m1 = 1;
+    d.out_s0 = n_out;
+    d.out_s1 = 0;
+    d.residual = residual ? d_res : nullptr;
+    d.alpha = alpha;
+    const GemmPlan plan = make_gemm_plan(d);
+    run_gemm(plan, nullptr);
+    B200_CUDA(cudaDeviceSynchronize());
+    B200_CUDA(cudaMemcpy(c, d_c, out_bytes, cudaMemcpyDeviceToHost));
 }
 
 }  // namespace b200

@@ -1,5 +1,5 @@
-// wgmma GEMM with fused epilogue:  out[row(g)][n] = act( sum_k A[g][k] * W[n][k] + bias[n] ), fp16 in/out,
-// fp32 accumulation in registers.  See gemm.cu.
+// wgmma GEMM with fused epilogue:  out[row(g)][n] = act( sum_k A[g][k] * W[n][k] + bias[n] ), fp16 in/out (or E4M3
+// operands, GemmDesc::fp8), fp32 accumulation in registers.  See gemm.cu.
 #pragma once
 
 #include "tc.cuh"
@@ -17,21 +17,24 @@ enum GemmAct : int {
 };
 
 struct GemmDesc {
+    // fp8 = 1: A and W are E4M3 bytes (K a multiple of 128, one 128-byte TMA box row per K block), and the SwiGLU epilogue
+    // writes E4M3; every other epilogue writes fp16.  Only GEMM_ACT_NONE and GEMM_ACT_SWIGLU have E4M3 forms.
+    int fp8 = 0;
     // A: logical [batches][rows_per_batch][K] fp16, K contiguous; row/batch strides in elements
-    const __half* a = nullptr;
+    const void* a = nullptr;
     int batches = 1;
     int rows_per_batch = 0;
     int64_t a_row_stride = 0;
     int64_t a_batch_stride = 0;
     // W: [N][K] fp16 (K contiguous, row stride = K_pad)
-    const __half* w = nullptr;
+    const void* w = nullptr;
     int N = 0;
-    int K = 0;  // multiple of 64 (pad weights with zeros)
+    int K = 0;  // multiple of 64 (128 for fp8; pad weights with zeros)
     int a_inner = 0;  // extent of A's K dimension in the tensor map (0 = K); elements beyond read as zero
     const float* bias = nullptr;
     int act = GEMM_ACT_NONE;
     // output: global row g = batch * rows_per_batch + row  ->  out + (g / out_m1) * out_s0 + (g % out_m1) * out_s1
-    __half* out = nullptr;
+    void* out = nullptr;   // fp16, or E4M3 bytes (fp8 SwiGLU)
     int64_t out_m1 = 1;
     int64_t out_s0 = 0;
     int64_t out_s1 = 0;

@@ -169,6 +169,26 @@ __device__ __forceinline__ void wgmma_m64n32k16(float* d, uint64_t adesc, uint64
             : "l"(adesc), "l"(bdesc), "r"((uint32_t)accumulate)
             : "memory");
 }
+// The same tile for E4M3 operands: D[64 x 32] (+)= A[64 x 32] B[32 x 32]^T, K-major (the only layout 8-bit wgmma takes),
+// fp32 accumulate.  32 E4M3 along K are 32 B, so stepping K inside the swizzle row is +2 in the address field as for
+// fp16; the accumulator fragment layout is that of wgmma_m64n32k16.
+__device__ __forceinline__ void wgmma_m64n32k32_e4m3(float* d, uint64_t adesc, uint64_t bdesc, bool accumulate) {
+    asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %18, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k32.f32.e4m3.e4m3 "
+            "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+              "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(adesc), "l"(bdesc), "r"((uint32_t)accumulate)
+            : "memory");
+}
+// Two fp32 values to E4M3 (round to nearest even; beyond +-448 saturates to +-448, NaN stays NaN): lo in the low byte.
+__device__ __forceinline__ uint16_t cvt_e4m3x2(float lo, float hi) {
+    uint16_t r;
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+    return r;
+}
 
 // ---------------------------------------------------------------- warp MMA (mma.sync) and ldmatrix
 // The latency-bound kernels (recurrence, conv2, attention) work on warp-sized tiles with the operands in registers.
@@ -212,10 +232,11 @@ __device__ __forceinline__ uint32_t sw128_offset(int row, int chunk16) {
 }  // namespace tc
 
 // ---------------------------------------------------------------- host: tensor maps
-// cuTensorMapEncodeTiled through the runtime's driver entry point (no link dependency on libcuda).
+// cuTensorMapEncodeTiled through the runtime's driver entry point (no link dependency on libcuda).  Elements are fp16, or
+// bytes (E4M3) when elem_bytes == 1; a box row of 128 bytes gets the 128-byte swizzle.
 CUtensorMap make_tmap_2d(const void* base, uint64_t inner, uint64_t outer, uint64_t outer_stride_bytes, uint32_t box_inner,
-                         uint32_t box_outer);
+                         uint32_t box_outer, uint32_t elem_bytes = 2);
 CUtensorMap make_tmap_3d(const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t s1_bytes, uint64_t s2_bytes,
-                         uint32_t b0, uint32_t b1, uint32_t b2);
+                         uint32_t b0, uint32_t b1, uint32_t b2, uint32_t elem_bytes = 2);
 
 }  // namespace b200

@@ -14,6 +14,11 @@
 // Activations are NTC fp16.  Every conv after the first is a strided GEMM over the zero-padded NTC buffer of
 // the previous layer (row stride = stride * C_in), all projections are wgmma GEMMs; the residual stream is
 // x <- RMSNorm(sublayer(x) + alpha * x) with the "+ alpha * x" fused into the GEMM epilogue.
+//
+// Precision B200_TX_FP8_FFN (the reference's koi_use_f8 = 1, koi_use_i8 = 0 configuration, TxModules.cpp:477-479, 560-575,
+// 596-697): fc1 and fc2 take E4M3 operands.  norm1 is an explicit pass that writes the fp16 row (fc2's residual) and its
+// E4M3 copy (fc1's A); fc1 + SwiGLU writes E4M3 (fc2's A); fc2 writes fp16.  The fp16 weights the reference keeps (QKV,
+// out_proj, both RMSNorm gains) lose their low 4 mantissa bits first (remove_bits, TxModules.cpp:104-111, 443-453).
 #include "engine.h"
 #include "gemm.h"
 #include "nvtx.h"
@@ -77,8 +82,10 @@ __global__ void __launch_bounds__(256) tx_conv1_kernel(const Conv1Params p) {
 // consecutive columns from i * dim / 32 (dim a multiple of 128, so whole 8-byte groups).  The row is read twice (sum of
 // squares, then the scaled store) rather than held in registers, so one kernel serves every width.
 // ------------------------------------------------------------------------------------------------
+// out8 (optional): the E4M3 cast of the fp16 values written to out, same layout (fc1's A in the fp8_ffn precision).
 __global__ void __launch_bounds__(256) rmsnorm_kernel(const __half* __restrict__ in, __half* __restrict__ out,
-                                                      const float* __restrict__ w, long long rows, int dim) {
+                                                      const float* __restrict__ w, long long rows, int dim,
+                                                      uint8_t* __restrict__ out8) {
     const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (row >= rows) return;
@@ -109,6 +116,11 @@ __global__ void __launch_bounds__(256) rmsnorm_kernel(const __half* __restrict__
             o2[j] = __floats2half2_rn(a.x * rstd * __ldg(w + c), a.y * rstd * __ldg(w + c + 1));
         }
         *reinterpret_cast<uint2*>(dst + i) = *reinterpret_cast<uint2*>(o2);
+        if (out8) {
+            const float2 f0 = __half22float2(o2[0]), f1 = __half22float2(o2[1]);
+            const uint32_t q = (uint32_t)tc::cvt_e4m3x2(f0.x, f0.y) | ((uint32_t)tc::cvt_e4m3x2(f1.x, f1.y) << 16);
+            *reinterpret_cast<uint32_t*>(out8 + row * dim + lane * per + i) = q;
+        }
     }
 }
 
@@ -337,6 +349,7 @@ void launch_attention(const CUtensorMap& qkv_map, const AttnTcParams& p, cudaStr
 // ------------------------------------------------------------------------------------------------
 struct TxLayerWeights {
     __half *wqkv = nullptr, *wo = nullptr, *w1 = nullptr, *w2 = nullptr;
+    uint8_t *w1_e4m3 = nullptr, *w2_e4m3 = nullptr;   // fp8_ffn: fc1 (interleaved rows) and fc2 as E4M3 (w1, w2 unused)
     float *bo = nullptr, *n1 = nullptr, *n2 = nullptr;
 };
 
@@ -352,6 +365,7 @@ public:
         GemmPlan qkv, out_proj, fc1, fc2;
         const float *n1, *n2;
     };
+    std::string info() const override { return fp8 ? "tx.fp8_ffn=1" : std::string(); }
     std::vector<Layer> layers;
     GemmPlan upsample, crf;
     CUtensorMap qkv_map;       // qkv as [N*T][3*H*64], box 64 x 128 (Q, K and V tiles of the tensor-core attention)
@@ -362,6 +376,9 @@ public:
     int norm_dim = 0;   // d_model: row width of the separate RMSNorm pass
     int n_launches = 0;
     bool fold_norm = true;
+    bool fp8 = false;           // fp8_ffn: explicit norm1 pass writing fp16 (norm_out) and E4M3 (norm_out8), E4M3 fc1 / fc2
+    __half* norm_out = nullptr;
+    uint8_t* norm_out8 = nullptr;
 };
 
 class TxModel final : public Model {
@@ -373,6 +390,7 @@ public:
                                            size_t ws_bytes) override;
     b200_model_desc desc;
     bool fold_norm = true;   // B200_TX_RMSNORM_PASS=1: separate RMSNorm kernel after every sub-layer (A/B comparisons)
+    bool fp8 = false;        // desc.tx_precision == B200_TX_FP8_FFN (norm2 stays folded; the RMSNorm-pass option is ignored)
     float* conv1_w = nullptr;
     std::vector<__half*> conv_w;  // conv 2..n  [C_out][W*C_in]
     std::vector<float*> conv_b;
@@ -406,13 +424,17 @@ TxModel::Shapes TxModel::shapes(int T_in) const {
 }
 
 TxModel::TxModel(const b200_model_desc& d, const b200_tensor* tensors, int n) : desc(d) {
-    if (const char* e = std::getenv("B200_TX_RMSNORM_PASS")) fold_norm = std::atoi(e) == 0;
+    fp8 = d.tx_precision == B200_TX_FP8_FFN;
+    if (const char* e = std::getenv("B200_TX_RMSNORM_PASS"); e && !fp8) fold_norm = std::atoi(e) == 0;
     // the shapes the kernels handle: head dimension 64 (attention, RoPE epilogue), d_model in whole 128-column tiles (the
     // folded RMSNorm's partial sums), K of the fc2 GEMM in whole 64-wide blocks, key bands of at most AT_MAXBLK blocks
     if (d.nhead < 1 || d.d_model != ATT_D * d.nhead) throw Unsupported("transformer path needs d_model == 64 * nhead (head dimension 64)");
     if (d.d_model % 128 != 0 || d.d_model > 1536) throw Unsupported("transformer path needs d_model a multiple of 128 and at most 1536");
     if (d.dim_feedforward < 64 || d.dim_feedforward % 64 != 0) throw Unsupported("transformer path needs dim_feedforward a multiple of 64");
     check_attention_window(d.attn_window_upper, d.attn_window_lower);
+    if (fp8 && d.dim_feedforward % 128 != 0) {
+        throw Unsupported("fp8_ffn precision needs dim_feedforward a multiple of 128 (fc2's K in whole 128-byte E4M3 blocks)");
+    }
     if (d.num_convs < 2 || d.convs[0].insize != 1 || d.convs[0].stride != 1 || d.convs[0].winlen > 9 || d.convs[0].size % 8) {
         throw Unsupported("transformer conv stack shape not supported");
     }
@@ -461,15 +483,33 @@ TxModel::TxModel(const b200_model_desc& d, const b200_tensor* tensors, int n) : 
         return out;
     };
     const float* prev_gain = nullptr;   // norm2 gain of the previous layer (none before layer 0: the conv output is used as is)
+    // fp8_ffn: the model as the reference holds it, fp16 (CudaCaller.cpp:167), with remove_bits applied to the fp16 weights
+    // it keeps; E4M3 weights are cast from the fp16 values.  The gains are rounded before they are folded into columns.
+    std::vector<std::vector<float>> rounded;   // this layer's weights as the engine uses them (rounded in fp8_ffn)
+    std::vector<float> gain2;                  // storage of prev_gain
+    auto rb = [&](const float* v, size_t cnt) -> const float* {
+        rounded.push_back(fp8 ? fp16_remove_bits(v, cnt, 4) : std::vector<float>(v, v + cnt));
+        return rounded.back().data();
+    };
+    auto up8 = [&](const float* v, size_t cnt) {
+        std::vector<uint8_t> q(cnt);
+        for (size_t i = 0; i < cnt; ++i) q[i] = e4m3_from_f16_bits(f16_bits(v[i]));
+        void* p = nullptr;
+        B200_CUDA(cudaMalloc(&p, cnt));
+        owned.push_back(p);
+        B200_CUDA(cudaMemcpy(p, q.data(), cnt, cudaMemcpyHostToDevice));
+        return static_cast<uint8_t*>(p);
+    };
     for (int l = 0; l < d.depth; ++l) {
         const std::string pfx = "transformer_encoder." + std::to_string(l) + ".";
         TxLayerWeights lw;
-        const float* n1 = find_tensor(tensors, n, pfx + "norm1.weight.tensor").data;
-        const float* n2 = find_tensor(tensors, n, pfx + "norm2.weight.tensor").data;
-        const auto& wqkv = find_tensor(tensors, n, pfx + "self_attn.Wqkv.weight.tensor");
-        lw.wqkv = up16(fold_norm ? fold(wqkv.data, (size_t)3 * dm, prev_gain) : std::vector<float>(wqkv.data, wqkv.data + (size_t)3 * dm * dm));
-        const auto& wo = find_tensor(tensors, n, pfx + "self_attn.out_proj.weight.tensor");
-        lw.wo = up16(std::vector<float>(wo.data, wo.data + (size_t)dm * dm));
+        const float* n1 = rb(find_tensor(tensors, n, pfx + "norm1.weight.tensor").data, dm);
+        const float* n2 = rb(find_tensor(tensors, n, pfx + "norm2.weight.tensor").data, dm);
+        const auto& wqkv_t = find_tensor(tensors, n, pfx + "self_attn.Wqkv.weight.tensor");
+        const float* wqkv = rb(wqkv_t.data, (size_t)3 * dm * dm);
+        lw.wqkv = up16(fold_norm ? fold(wqkv, (size_t)3 * dm, prev_gain) : std::vector<float>(wqkv, wqkv + (size_t)3 * dm * dm));
+        const float* wo = rb(find_tensor(tensors, n, pfx + "self_attn.out_proj.weight.tensor").data, (size_t)dm * dm);
+        lw.wo = up16(std::vector<float>(wo, wo + (size_t)dm * dm));
         lw.bo = up32(find_tensor(tensors, n, pfx + "self_attn.out_proj.bias.tensor").data, dm);
         // fc1 rows [y(0..ff) | gate(0..ff)] (TxModules.cpp:170-176) interleaved to (y_j, gate_j) pairs
         const auto& w1 = find_tensor(tensors, n, pfx + "ff.fc1.weight.tensor");
@@ -478,13 +518,21 @@ TxModel::TxModel(const b200_model_desc& d, const b200_tensor* tensors, int n) : 
             std::memcpy(&w1i[(size_t)(2 * j) * dm], &w1.data[(size_t)j * dm], sizeof(float) * dm);
             std::memcpy(&w1i[(size_t)(2 * j + 1) * dm], &w1.data[(size_t)(ff + j) * dm], sizeof(float) * dm);
         }
-        lw.w1 = up16(fold_norm ? fold(w1i.data(), (size_t)2 * ff, n1) : w1i);
-        prev_gain = n2;
         const auto& w2 = find_tensor(tensors, n, pfx + "ff.fc2.weight.tensor");
-        lw.w2 = up16(std::vector<float>(w2.data, w2.data + (size_t)dm * ff));
-        lw.n1 = up32(find_tensor(tensors, n, pfx + "norm1.weight.tensor").data, dm);
-        lw.n2 = up32(find_tensor(tensors, n, pfx + "norm2.weight.tensor").data, dm);
+        if (fp8) {
+            // norm1 is an explicit pass here, so no gain goes into fc1's columns
+            lw.w1_e4m3 = up8(w1i.data(), w1i.size());
+            lw.w2_e4m3 = up8(w2.data, (size_t)dm * ff);
+        } else {
+            lw.w1 = up16(fold_norm ? fold(w1i.data(), (size_t)2 * ff, n1) : w1i);
+            lw.w2 = up16(std::vector<float>(w2.data, w2.data + (size_t)dm * ff));
+        }
+        lw.n1 = up32(n1, dm);
+        lw.n2 = up32(n2, dm);
         layers.push_back(lw);
+        gain2.assign(n2, n2 + dm);
+        prev_gain = gain2.data();
+        rounded.clear();
     }
     {
         const auto& tw = find_tensor(tensors, n, "upsample.linear.weight.tensor");
@@ -586,7 +634,7 @@ std::unique_ptr<ForwardPlan> TxModel::make_plan(int N, int T_in, const __half* s
         g.out_s1 = c.size;
         plan->convs.push_back(make_gemm_plan(g));
     }
-    auto dense = [&](const __half* a, int K, const __half* w, int Nout, const float* bias, int act, __half* out, int ld_out,
+    auto dense = [&](const void* a, int K, const void* w, int Nout, const float* bias, int act, void* out, int ld_out,
                      const __half* residual, float alpha) {
         GemmDesc g{};
         g.a = a;
@@ -618,7 +666,24 @@ std::unique_ptr<ForwardPlan> TxModel::make_plan(int N, int T_in, const __half* s
     for (int l = 0; l < desc.depth; ++l) {
         const auto& lw = layers[l];
         TxPlan::Layer L;
-        if (fold_norm) {
+        if (fp8) {
+            // qkv and out_proj as in the folded fp16 layout; norm1 -> att (fp16) + qkv's buffer (E4M3, free once attention has
+            // read it); fc1 + SwiGLU -> hid (E4M3); fc2 -> x (fp16, + alpha * att) with the partial sums for the folded norm2
+            const bool first = l == 0;
+            GemmDesc q = dense(x, dm, lw.wqkv, dqkv, nullptr, GEMM_ACT_ROPE, qkv, dqkv, nullptr, 0.0f);
+            if (!first) { q.a_ss = ss_a; q.a_ss_parts = ssp; }
+            L.qkv = make_gemm_plan(q);
+            GemmDesc o = dense(att, dm, lw.wo, dm, lw.bo, GEMM_ACT_NONE, y, dm, x, desc.deepnorm_alpha);
+            if (!first) { o.res_ss = ss_a; o.res_ss_parts = ssp; o.res_gain = layers[l - 1].n2; }
+            L.out_proj = make_gemm_plan(o);
+            GemmDesc f1 = dense(qkv, dm, lw.w1_e4m3, 2 * ff, nullptr, GEMM_ACT_SWIGLU, hid, ff, nullptr, 0.0f);
+            f1.fp8 = 1;
+            L.fc1 = make_gemm_plan(f1);
+            GemmDesc f2 = dense(hid, ff, lw.w2_e4m3, dm, nullptr, GEMM_ACT_NONE, x, dm, att, desc.deepnorm_alpha);
+            f2.fp8 = 1;
+            f2.out_ss = ss_a;
+            L.fc2 = make_gemm_plan(f2);
+        } else if (fold_norm) {
             // x holds u_prev (un-normalised, ss_a) except before layer 0, y will hold u_mid (ss_b)
             const bool first = l == 0;
             GemmDesc q = dense(x, dm, lw.wqkv, dqkv, nullptr, GEMM_ACT_ROPE, qkv, dqkv, nullptr, 0.0f);
@@ -676,7 +741,10 @@ std::unique_ptr<ForwardPlan> TxModel::make_plan(int N, int T_in, const __half* s
     plan->H = desc.nhead;
     plan->norm_dim = dm;
     plan->fold_norm = fold_norm;
-    plan->n_launches = 1 + (desc.num_convs - 1) + desc.depth * (fold_norm ? 5 : 7) + 2;
+    plan->fp8 = fp8;
+    plan->norm_out = att;
+    plan->norm_out8 = reinterpret_cast<uint8_t*>(qkv);
+    plan->n_launches = 1 + (desc.num_convs - 1) + desc.depth * (fp8 ? 6 : fold_norm ? 5 : 7) + 2;
     return plan;
 }
 
@@ -711,9 +779,13 @@ void TxPlan::run(cudaStream_t stream, ProfileSink* prof) {
             run_gemm(L.out_proj, stream);
             if (prof) prof->mark("out_proj_gemm", stream);
         }
-        if (!fold_norm) {
+        if (fp8) {
             NvtxRange r("LNORM1");
-            rmsnorm_kernel<<<norm_grid, 256, 0, stream>>>(y, x, L.n1, rows, norm_dim);
+            rmsnorm_kernel<<<norm_grid, 256, 0, stream>>>(y, norm_out, L.n1, rows, norm_dim, norm_out8);
+            if (prof) prof->mark("rmsnorm_e4m3", stream);
+        } else if (!fold_norm) {
+            NvtxRange r("LNORM1");
+            rmsnorm_kernel<<<norm_grid, 256, 0, stream>>>(y, x, L.n1, rows, norm_dim, nullptr);
             if (prof) prof->mark("rmsnorm", stream);
         }
         {
@@ -728,7 +800,7 @@ void TxPlan::run(cudaStream_t stream, ProfileSink* prof) {
         }
         if (!fold_norm) {
             NvtxRange r("LNORM2");
-            rmsnorm_kernel<<<norm_grid, 256, 0, stream>>>(y, x, L.n2, rows, norm_dim);
+            rmsnorm_kernel<<<norm_grid, 256, 0, stream>>>(y, x, L.n2, rows, norm_dim, nullptr);
             if (prof) prof->mark("rmsnorm", stream);
         }
     }
@@ -755,6 +827,51 @@ std::unique_ptr<Model> make_tx_model(const b200_model_desc& desc, const b200_ten
 // ------------------------------------------------------------------------------------------------
 // test hook: host buffers in, host buffer out, the model's attention launch in between
 // ------------------------------------------------------------------------------------------------
+// ------------------------------------------------------------------------------------------------
+// host-side rounding of the fp8_ffn weights
+// ------------------------------------------------------------------------------------------------
+uint16_t f16_bits(float v) {
+    const __half h = __float2half_rn(v);
+    uint16_t b;
+    std::memcpy(&b, &h, 2);
+    return b;
+}
+
+static float f16_value(uint16_t b) {
+    __half h;
+    std::memcpy(&h, &b, 2);
+    return __half2float(h);
+}
+
+uint16_t remove_bits_f16(uint16_t b, int bits) {
+    if (bits <= 0) return b;
+    // the reference's integer trick on the int16 view: add half an ulp of the kept mantissa, clear the low bits.  Carries
+    // run into the exponent, so the values next to +-65504 become +-inf (the reference's own TODO, TxModules.cpp:107).
+    return (uint16_t)((b + (1u << (bits - 1))) & (0xffffu & ~((1u << bits) - 1u)));
+}
+
+std::vector<float> fp16_remove_bits(const float* v, size_t n, int bits) {
+    std::vector<float> out(n);
+    for (size_t i = 0; i < n; ++i) out[i] = f16_value(remove_bits_f16(f16_bits(v[i]), bits));
+    return out;
+}
+
+uint8_t e4m3_from_f16_bits(uint16_t b) {
+    // torch's float -> float8_e4m3fn cast of the fp16 value: round to nearest even; |x| >= 480 (after rounding beyond 448),
+    // inf and NaN give NaN (0x7f with the sign), there is no saturation
+    const float f = f16_value(b);
+    uint32_t u;
+    std::memcpy(&u, &f, 4);
+    const uint8_t sign = (uint8_t)((b >> 8) & 0x80u);   // from the fp16 bits: the host fp16 -> float conversion drops a NaN's sign
+    u &= 0x7fffffffu;
+    if (u >= 0x43f00000u) return sign | 0x7f;                              // 480
+    if (u < 0x3c800000u) return sign | (uint8_t)std::nearbyint(std::fabs(f) * 512.0f);   // below 2^-6: multiples of 2^-9
+    uint32_t keep = u >> 20;                                                 // sign-less exponent and 3 mantissa bits
+    const uint32_t rest = u & 0xfffffu;
+    if (rest > 0x80000u || (rest == 0x80000u && (keep & 1u))) ++keep;
+    return sign | (uint8_t)(keep - ((127u - 7u) << 3));
+}
+
 void test_attention_host(int device, const uint16_t* qkv, int N, int T, int H, int win_upper, int win_lower, uint16_t* out) {
     if (N < 1 || T < 1 || H < 1 || H > 65535 || N > 65535) throw std::invalid_argument("test_attention: bad N, T or H");
     check_attention_window(win_upper, win_lower);

@@ -42,8 +42,12 @@ class ModelDesc(C.Structure):
         ("attn_window_upper", C.c_int32), ("attn_window_lower", C.c_int32),
         ("upsample_scale", C.c_int32), ("max_seq_len", C.c_int32),
         ("deepnorm_alpha", C.c_float), ("theta", C.c_float), ("tx_crf_scale", C.c_float),
-        ("lstm_inner_dim", C.c_int32),
+        ("lstm_inner_dim", C.c_int32), ("tx_precision", C.c_int32),
     ]
+
+
+# b200_model_desc.tx_precision
+TX_PRECISIONS = {"fp16": 0, "fp8_ffn": 1}
 
 
 class Tensor(C.Structure):
@@ -91,7 +95,7 @@ EXPORTS = [
     "b200_runner_set_decoder_options", "b200_runner_batch_size", "b200_runner_chunk_size", "b200_runner_out_len",
     "b200_runner_accept_chunk_f16", "b200_runner_accept_chunk_f32", "b200_runner_input", "b200_runner_call_chunks",
     "b200_runner_upload", "b200_runner_step_device", "b200_runners_step_device", "b200_runner_forward_scores", "b200_runner_profile", "b200_runner_plan_info", "b200_runner_debug_read_workspace", "b200_decode_scores",
-    "b200_test_gemm", "b200_test_attention", "b200_generate_chunks", "b200_stitch_chunks", "b200_runner_accept_raw_chunk",
+    "b200_test_gemm", "b200_test_gemm_fp8", "b200_test_to_e4m3", "b200_test_remove_bits", "b200_test_attention", "b200_generate_chunks", "b200_stitch_chunks", "b200_runner_accept_raw_chunk",
     "b200_runner_debug_read_input", "b200_engine_runner_bytes", "b200_engine_benchmark_batch_sizes",
     "b200_select_batch_size", "b200_generate_variable_chunks", "b200_engine_terminate", "b200_engine_restart",
     "b200_engine_set_low_latency", "b200_engine_is_low_latency", "b200_engine_batch_timeouts_ms",
@@ -173,6 +177,9 @@ def load_library() -> C.CDLL:
     lib.b200_runner_debug_read_workspace.argtypes = [vp, C.c_uint64, C.c_uint64, vp]
     lib.b200_test_gemm.argtypes = [i32, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.b200_test_attention.argtypes = [i32, vp, i32, i32, i32, i32, i32, vp]
+    lib.b200_test_gemm_fp8.argtypes = [i32, vp, vp, i32, i32, i32, i32, vp, f32, vp]
+    lib.b200_test_to_e4m3.argtypes = [vp, C.c_int64, vp]
+    lib.b200_test_remove_bits.argtypes = [vp, C.c_int64, i32, vp]
     u64 = C.c_uint64
     lib.b200_generate_chunks.argtypes = [u64, u64, u64, u64, C.POINTER(u64), u64, C.POINTER(u64)]
     lib.b200_generate_variable_chunks.argtypes = [u64, u64, u64, u64, C.POINTER(u64), u64, C.POINTER(u64)]
@@ -202,8 +209,12 @@ def check(status: int) -> None:
         raise B200Error(status, load_library().b200_last_error().decode())
 
 
-def model_desc_from_config(cfg: BasecallModelConfig) -> ModelDesc:
+def model_desc_from_config(cfg: BasecallModelConfig, precision: str = "fp16") -> ModelDesc:
+    """precision: the transformer precision, "fp16" (default) or "fp8_ffn" (E4M3 feed-forward GEMMs, b200call.h)."""
+    if precision not in TX_PRECISIONS:
+        raise ValueError(f"precision must be one of {sorted(TX_PRECISIONS)}, got {precision!r}")
     d = ModelDesc()
+    d.tx_precision = TX_PRECISIONS[precision]
     d.model_type = 1 if cfg.is_tx_model else 0
     d.num_convs = len(cfg.convs)
     for i, c in enumerate(cfg.convs):
@@ -274,6 +285,41 @@ def test_gemm(a: np.ndarray, b: np.ndarray, bias: np.ndarray | None, activation:
         bias_p = bias.ctypes.data
     check(lib.b200_test_gemm(device, a.ctypes.data, b.ctypes.data, bias_p, M, N, K, activation, c.ctypes.data))
     return c
+
+
+def test_gemm_fp8(a: np.ndarray, b: np.ndarray, activation: int = -1, residual: np.ndarray | None = None,
+                  alpha: float = 0.0, device: int = 0):
+    """The E4M3 GEMM on host data: a [M, K], b [N, K] E4M3 bytes (uint8) -> fp16 [M, N] (activation -1, optionally
+    + alpha * residual [M, N] fp16) or E4M3 bytes [M, N / 2] (activation 4, SwiGLU)."""
+    lib = load_library()
+    a = np.ascontiguousarray(a, np.uint8)
+    b = np.ascontiguousarray(b, np.uint8)
+    M, K = a.shape
+    N = b.shape[0]
+    c = np.empty((M, N // 2), np.uint8) if activation == 4 else np.empty((M, N), np.float16)
+    res_p = None
+    if residual is not None:
+        residual = np.ascontiguousarray(residual, np.float16)
+        assert residual.shape == (M, N)
+        res_p = residual.ctypes.data
+    check(lib.b200_test_gemm_fp8(device, a.ctypes.data, b.ctypes.data, M, N, K, activation, res_p, alpha, c.ctypes.data))
+    return c
+
+
+def to_e4m3(x: np.ndarray) -> np.ndarray:
+    """The engine's host cast of fp16 values to E4M3 bytes (no device needed)."""
+    h = np.ascontiguousarray(x, np.float16)
+    out = np.empty(h.shape, np.uint8)
+    check(load_library().b200_test_to_e4m3(h.ctypes.data, h.size, out.ctypes.data))
+    return out
+
+
+def remove_bits(x: np.ndarray, bits: int = 4) -> np.ndarray:
+    """The engine's host remove_bits on fp16 values (no device needed); returns fp16."""
+    h = np.ascontiguousarray(x, np.float16)
+    out = np.empty(h.shape, np.float16)
+    check(load_library().b200_test_remove_bits(h.ctypes.data, h.size, bits, out.ctypes.data))
+    return out
 
 
 def test_attention(qkv: np.ndarray, win_upper: int, win_lower: int, device: int = 0):

@@ -36,11 +36,13 @@ class B200Caller:
     """One model replica on one GPU (CudaCaller, dorado/basecall/CudaCaller.cpp:149-202)."""
 
     def __init__(self, cfg: BasecallModelConfig, weights: dict, device: int = 0, low_latency: bool = False,
-                 num_runners: int = 2):
+                 num_runners: int = 2, precision: str = "fp16"):
+        """precision: transformer precision, "fp16" or "fp8_ffn" (fc1 / fc2 on E4M3 operands; include/b200call.h)."""
         self.cfg = cfg
         self.device = device
+        self.precision = precision
         lib = L.load_library()
-        desc = L.model_desc_from_config(cfg)
+        desc = L.model_desc_from_config(cfg, precision)
         self._keep = []
         arr = (L.Tensor * len(weights))()
         for i, (name, w) in enumerate(weights.items()):
@@ -127,10 +129,10 @@ class B200Pool:
     `runners_per_device` runners each, one pinned host thread per runner, batches taken from one shared cursor."""
 
     def __init__(self, cfg: BasecallModelConfig, weights: dict, devices, runners_per_device: int, batch_size: int,
-                 chunk_size: int):
+                 chunk_size: int, precision: str = "fp16"):
         self.cfg = cfg
         self._lib = lib = L.load_library()
-        desc = L.model_desc_from_config(cfg)
+        desc = L.model_desc_from_config(cfg, precision)
         arr, keep = _weight_array(weights)
         devs = (C.c_int32 * len(devices))(*devices)
         self.chunk_size = cfg.normalise_chunk_size(chunk_size)

@@ -18,6 +18,7 @@
 #include "basecall/ModelRunnerBase.h"
 #include "basecall/crf_utils.h"
 #include "config/BasecallModelConfig.h"
+#include "utils/dev_utils.h"
 
 #include <ATen/ATen.h>
 
@@ -68,6 +69,12 @@ public:
             d.max_seq_len = tx.max_seq_len;
             d.upsample_scale = model_config.tx->upsample.scale_factor;
             d.tx_crf_scale = model_config.tx->crf.scale;
+            // The reference's dev option (TxModules.cpp:477-479): koi_use_f8=1 runs fc1 / fc2 on E4M3 operands with
+            // remove_bits = 4 on the fp16 weights it keeps (b200call.h, tx_precision).  Off unless asked for here: the fp16
+            // path is the one held to the oracle.  koi_use_i8 and other remove_bits values have no counterpart.
+            if (utils::get_dev_opt<bool>("koi_use_f8", false)) {
+                d.tx_precision = B200_TX_FP8_FFN;
+            }
         }
         // Weights: the reference's own loader (crf_utils.cpp:26-150) gives the tensors in file-list order; the
         // engine wants them as named host fp32 arrays.

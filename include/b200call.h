@@ -37,6 +37,8 @@ typedef enum b200_status {
 enum { B200_ACT_SWISH = 0, B200_ACT_SWISH_CLAMP = 1, B200_ACT_TANH = 2 };
 /* model family */
 enum { B200_MODEL_LSTM = 0, B200_MODEL_TX = 1 };
+/* transformer precision (b200_model_desc.tx_precision) */
+enum { B200_TX_FP16 = 0, B200_TX_FP8_FFN = 1 };
 
 /* config::ConvParams (dorado/config/include/config/common.h) */
 typedef struct b200_conv_desc {
@@ -71,6 +73,15 @@ typedef struct b200_model_desc {
      * as dn_weight_ih/hh [K, C], up_weight_ih/hh [4C, K], up_bias_ih/hh [4C]; the engine folds up x dn into the [4C, C] gate
      * matrices once at load time and runs the LSTM kernels unchanged. */
     int32_t lstm_inner_dim;
+    /* Transformer precision.  B200_TX_FP16 (0, what a zero-initialised descriptor gets): every GEMM in fp16 with fp32
+     * accumulation.  B200_TX_FP8_FFN (1): the reference's koi_use_f8 = 1, koi_use_i8 = 0 configuration
+     * (dorado/nn/TxModules.cpp:477-479, 560-575, 596-697).  The weights are rounded to fp16 first; QKV, out_proj and both
+     * RMSNorm gains then lose their low 4 mantissa bits (remove_bits = 4); fc1 and fc2 weights are cast to E4M3 without a
+     * scale.  norm1 writes its output in fp16 and as an E4M3 copy, fc1 + SwiGLU reads the copy and writes E4M3, fc2 reads
+     * that and writes fp16; both accumulate in fp32.  Shapes: those above, and dim_feedforward a multiple of 128 (fc2's K
+     * in whole 128-byte E4M3 blocks; the engine does not pad it): others return B200_ERR_UNSUPPORTED.  On an LSTM model,
+     * or any other value, b200_engine_create returns B200_ERR_INVALID.  b200_runner_plan_info reports "tx.fp8_ffn=1". */
+    int32_t tx_precision;
 } b200_model_desc;
 
 /* Host fp32 tensors, named and ordered as the reference's *.tensor files
@@ -437,6 +448,15 @@ B200_API int b200_modbase_runner_profile(b200_modbase_runner* runner, char* buf,
 B200_API int b200_modbase_runner_debug_read_workspace(b200_modbase_runner* runner, uint64_t offset, uint64_t bytes, void* dst);
 
 /* Kernel-level test hooks (host buffers; used by tests/ only). */
+/* The GEMM with E4M3 operands (A [M,K], W [N,K] bytes; K is zero-padded to a multiple of 128 inside).  activation -1:
+ * c = A W^T (+ alpha * residual when residual [M,N] fp16 is given), fp16 [M,N].  activation 4 (SwiGLU, columns (2i, 2i+1)
+ * = (y, gate)): c = E4M3 [M,N/2] of y * silu(gate). */
+B200_API int b200_test_gemm_fp8(int32_t device, const uint8_t* a, const uint8_t* b, int32_t M, int32_t N, int32_t K,
+                                int32_t activation, const uint16_t* residual, float alpha, void* c);
+/* Host only, no device: the fp8_ffn weight rounding.  to_e4m3: torch's float8_e4m3fn cast of each fp16 value (round to
+ * nearest even; NaN beyond the range).  remove_bits: the reference's (bits + 2^(b-1)) & ~(2^b - 1) on the int16 view. */
+B200_API int b200_test_to_e4m3(const uint16_t* f16, int64_t n, uint8_t* out);
+B200_API int b200_test_remove_bits(const uint16_t* f16, int64_t n, int32_t bits, uint16_t* out);
 B200_API int b200_test_gemm(int32_t device, const uint16_t* a /* [M,K] fp16 */, const uint16_t* b /* [N,K] fp16 */,
                             const float* bias /* [N] or NULL */, int32_t M, int32_t N, int32_t K, int32_t activation,
                             uint16_t* c /* [M,N] fp16 */);

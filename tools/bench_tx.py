@@ -2,8 +2,11 @@
 """Throughput of the transformer models on one GPU: sup@v5 (d_model 512, window (127, 128)) and the synthetic 1536-wide
 fixture (d_model 1536, 24 heads, window (255, 256), feed-forward 6144; see tests/test_tx1536_cpu.py).
 
-usage: python tools/bench_tx.py --model sup|tx1536 [--batch 128] [--chunksize 12288] [--runners 2] [--steps 10]
-       [--warmup 3]
+usage: python tools/bench_tx.py --model sup|tx1536 [--precision fp16|fp8_ffn] [--batch 128] [--chunksize 12288]
+       [--runners 2] [--steps 10] [--warmup 3]
+
+--precision fp8_ffn runs fc1 + SwiGLU and fc2 on E4M3 operands behind an explicit norm1 pass (include/b200call.h); their
+FLOP rates are then to be read against the data sheet's dense FP8 figure (1,979 TFLOP/s), also printed.
 
 Device-resident steps as bench.py times them (step i on runner i % R, each runner on its own stream), then one profiled
 forward + decode with an event after every launch.  Prints one JSON line: samples/s, the card (name, power limit, SM
@@ -24,6 +27,7 @@ ROOT = pathlib.Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
 
 DATASHEET_FP16_TFLOPS = 989.0
+DATASHEET_FP8_TFLOPS = 1979.0
 CONFIGS = ROOT / "tests" / "data" / "model_configs"
 MODELS = {"sup": CONFIGS / "dna_r10.4.1_e8.2_400bps_sup@v5.0.0", "tx1536": CONFIGS / "synthetic_tx1536@v0"}
 
@@ -73,6 +77,7 @@ def main():
     from dorado_b200.weights import synthetic_weights
     ap = argparse.ArgumentParser()
     ap.add_argument("--model", required=True, choices=list(MODELS))
+    ap.add_argument("--precision", default="fp16", choices=["fp16", "fp8_ffn"])
     ap.add_argument("--batch", type=int, default=128)
     ap.add_argument("--chunksize", type=int, default=12288)
     ap.add_argument("--runners", type=int, default=2)
@@ -84,7 +89,7 @@ def main():
 
     cfg = load_model_config(MODELS[args.model])
     N, R = args.batch, max(1, args.runners)
-    caller = B200Caller(cfg, synthetic_weights(cfg, 42), num_runners=R)
+    caller = B200Caller(cfg, synthetic_weights(cfg, 42), num_runners=R, precision=args.precision)
     runner_bytes = caller.runner_bytes(N, args.chunksize)
     runners = [B200ModelRunner(caller, N, args.chunksize) for _ in range(R)]
     T = runners[0].chunk_size()
@@ -108,15 +113,20 @@ def main():
         if k in prof:
             launches, t = prof[k]
             rates[k] = {"ms_per_launch": t / launches, "tflops": f * rows * launches / (t * 1e-3) / 1e12}
+    if "rmsnorm_e4m3" in prof:   # reads the fp16 row, writes it in fp16 and E4M3
+        launches, t = prof["rmsnorm_e4m3"]
+        rates["rmsnorm_e4m3"] = {"ms_per_launch": t / launches,
+                                 "gb_per_s": rows * cfg.tx.d_model * 5 * launches / (t * 1e-3) / 1e9}
     att_launches, att_ms = prof["tx_attention"]
     fps = flop_per_sample(cfg)
-    out = {"model": args.model, "d_model": cfg.tx.d_model, "nhead": cfg.tx.nhead, "attn_window": list(cfg.tx.attn_window),
+    out = {"model": args.model, "precision": args.precision, "d_model": cfg.tx.d_model, "nhead": cfg.tx.nhead, "attn_window": list(cfg.tx.attn_window),
            "batch": N, "chunk_samples": T, "tokens": tokens, "runners": R, "steps": args.steps,
            "runner_bytes": runner_bytes, "card": gpu,
            "samples_per_s": value, "ms_per_step": ms / args.steps,
            "flop_per_sample": fps, "flop_per_token_layer": flop_per_token_layer(cfg),
            "forward_tflops_per_s": fps * value / 1e12,
            "frac_of_datasheet_fp16": fps * value / 1e12 / DATASHEET_FP16_TFLOPS,
+           "datasheet_tflops": {"fp16": DATASHEET_FP16_TFLOPS, "fp8": DATASHEET_FP8_TFLOPS},
            "kernels_ms": {k: {"launches": n, "ms": round(t, 4)} for k, (n, t) in prof.items()},
            "kernel_rates": rates,
            "attention_ms_per_layer": att_ms / att_launches,
