@@ -1066,13 +1066,10 @@ size_t decode_max_blocks() {
     return (size_t)T;
 }
 
-size_t decode_scratch_bytes(int N, int T, int state_len, size_t* bwd_bytes, size_t* beam_bytes) {
+void carve_decode_scratch(Bump& b, int N, int T, int state_len, float** bwd, uint2** beam) {
     const size_t S = (size_t)1 << (2 * state_len);
-    const size_t b1 = ((size_t)N * (T + 1) * S * sizeof(float) + 255) & ~(size_t)255;
-    const size_t b2 = ((size_t)N * T * kBeamW * sizeof(uint2) + 255) & ~(size_t)255;
-    if (bwd_bytes) *bwd_bytes = b1;
-    if (beam_bytes) *beam_bytes = b2;
-    return b1 + b2;
+    *bwd = b.take<float>((size_t)N * (T + 1) * S * sizeof(float));
+    *beam = b.take<uint2>((size_t)N * T * kBeamW * sizeof(uint2));
 }
 
 int decode_launches(int state_len) { return state_len == 3 ? 2 : 3; }

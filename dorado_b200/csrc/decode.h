@@ -27,8 +27,8 @@ struct DecodeArgs {
     int runners;          // batches in flight on the device (Model::num_runners_hint; < 1 means 1): sizes the state_len 3 grid
     long long* dbg;  // optional clock64 timeline of chunk 0, state_len 4 and 5 (B200_DEBUG_BEAM_TIMELINE, test hook only); nullptr in production
     // scratch
-    float* bwd;   // decode_scratch_bytes() -> bwd_bytes
-    uint2* beam;  //                        -> beam_bytes
+    float* bwd;   // carve_decode_scratch()
+    uint2* beam;
     // outputs (device), rows of T
     uint8_t* moves;
     char* sequence;
@@ -37,7 +37,9 @@ struct DecodeArgs {
 };
 
 size_t decode_max_blocks();  // largest T the traceback kernel's shared-memory plan holds
-size_t decode_scratch_bytes(int N, int T, int state_len, size_t* bwd_bytes, size_t* beam_bytes);
+class Bump;
+// The decoder's scratch for N chunks of T blocks: backward scores [N][T + 1][4^state_len] and beam records [N][T][32]
+void carve_decode_scratch(Bump& b, int N, int T, int state_len, float** bwd, uint2** beam);
 int decode_launches(int state_len);  // kernels one decode_scores call launches
 struct ProfileSink;
 void decode_scores(const DecodeArgs& args, cudaStream_t stream, ProfileSink* prof = nullptr);

@@ -497,12 +497,15 @@ void test_gemm_host(int device, const uint16_t* a, const uint16_t* b, const floa
     require_sm90(device);
     const int Kp = (K + BK - 1) / BK * BK;
     const int n_out = activation == GEMM_ACT_SWIGLU ? N / 2 : N;
+    __half *d_a = nullptr, *d_w = nullptr, *d_c = nullptr;
+    float* d_bias = nullptr;
     Arena arena;
-    arena.reserve((size_t)M * Kp * 2 + (size_t)N * Kp * 2 + (size_t)N * 4 + (size_t)M * n_out * 2 + 4096);
-    auto* d_a = static_cast<__half*>(arena.take((size_t)M * Kp * 2));
-    auto* d_w = static_cast<__half*>(arena.take((size_t)N * Kp * 2));
-    auto* d_bias = static_cast<float*>(arena.take((size_t)N * 4));
-    auto* d_c = static_cast<__half*>(arena.take((size_t)M * n_out * 2));
+    arena.allocate([&](Bump& b) {
+        d_a = b.take<__half>((size_t)M * Kp * 2);
+        d_w = b.take<__half>((size_t)N * Kp * 2);
+        d_bias = b.take<float>((size_t)N * 4);
+        d_c = b.take<__half>((size_t)M * n_out * 2);
+    });
     B200_CUDA(cudaMemset(d_a, 0, (size_t)M * Kp * 2));
     B200_CUDA(cudaMemset(d_w, 0, (size_t)N * Kp * 2));
     B200_CUDA(cudaMemcpy2D(d_a, (size_t)Kp * 2, a, (size_t)K * 2, (size_t)K * 2, M, cudaMemcpyHostToDevice));
@@ -541,12 +544,16 @@ void test_gemm_fp8_host(int device, const uint8_t* a, const uint8_t* b, int M, i
     const bool swiglu = activation == GEMM_ACT_SWIGLU;
     const int n_out = swiglu ? N / 2 : N;
     const size_t out_bytes = (size_t)M * n_out * (swiglu ? 1 : 2);
+    uint8_t *d_a = nullptr, *d_w = nullptr;
+    __half* d_res = nullptr;
+    void* d_c = nullptr;
     Arena arena;
-    arena.reserve((size_t)M * Kp + (size_t)N * Kp + (size_t)M * N * 2 + out_bytes + 4096);
-    auto* d_a = static_cast<uint8_t*>(arena.take((size_t)M * Kp));
-    auto* d_w = static_cast<uint8_t*>(arena.take((size_t)N * Kp));
-    auto* d_res = static_cast<__half*>(arena.take((size_t)M * N * 2));
-    void* d_c = arena.take(out_bytes);
+    arena.allocate([&](Bump& b) {
+        d_a = b.take<uint8_t>((size_t)M * Kp);
+        d_w = b.take<uint8_t>((size_t)N * Kp);
+        d_res = b.take<__half>((size_t)M * N * 2);
+        d_c = b.take(out_bytes);
+    });
     B200_CUDA(cudaMemset(d_a, 0, (size_t)M * Kp));
     B200_CUDA(cudaMemset(d_w, 0, (size_t)N * Kp));
     B200_CUDA(cudaMemcpy2D(d_a, (size_t)Kp, a, (size_t)K, (size_t)K, M, cudaMemcpyHostToDevice));

@@ -55,15 +55,22 @@ struct LstmStackDesc {
     int num_layers = 0;
 };
 // The stack's slice of the caller's workspace: gx [T][Np][4C] (not for lstm_size 96), and for 768 / 1024 the group
-// counters and the error word of the grid recurrence
-size_t lstm_stack_workspace_bytes(int C, int num_layers, int T, int Np);
+// counters (one per 32 chunks and layer) and the error word of the grid recurrence
+struct LstmStackBuffers {
+    __half* gx = nullptr;
+    unsigned int* counters = nullptr;
+    size_t counter_bytes = 0;
+    int* error = nullptr;
+};
+class Bump;
+LstmStackBuffers carve_lstm_stack(Bump& b, int C, int num_layers, int T, int Np);
 
 // Every layer is lstm_layer_kernel (lstm_size 96), or the x-projection GEMM followed by lstm_rec_kernel (128 - 384) or by
 // one or more cooperative launches of lstm_grid_rec_kernel (768, 1024).  Built once per batch shape; reads
 // B200_DEBUG_LSTM_LAYERS, B200_CLUSTER_CHUNKS, B200_GRID_CHUNKS and B200_GRID_GROUPS then.
 class LstmStack {
 public:
-    LstmStack(const LstmStackDesc& d, void* ws);  // ws: lstm_stack_workspace_bytes, 256-byte aligned
+    LstmStack(const LstmStackDesc& d, const LstmStackBuffers& ws);  // ws: carved by carve_lstm_stack for the same shape
     ~LstmStack();
     LstmStack(const LstmStack&) = delete;
     LstmStack& operator=(const LstmStack&) = delete;
@@ -85,12 +92,10 @@ private:
     // chunks per CTA / cluster / group, groups per launch, launches per layer, CTAs per group
     int m_nb = 0, m_groups = 0, m_launches = 1, m_group_ctas = 1;
     std::vector<GemmPlan> m_gx_gemm;  // per layer (not for lstm_size 96)
-    __half* m_gx = nullptr;
+    // the counters are zeroed at the start of every run; a group whose step barrier timed out sets the error word
+    LstmStackBuffers m_ws;
     const int32_t* m_lens = nullptr;
-    unsigned int* m_counters = nullptr;  // lstm_size 768 / 1024: Np / 32 per layer, zeroed at the start of every run
-    size_t m_counter_bytes = 0;
-    int* m_error = nullptr;       // set by a group whose step barrier timed out
-    int* m_error_host = nullptr;  // pinned copy, written at the end of every run
+    int* m_error_host = nullptr;  // pinned copy of the error word, written at the end of every run
 };
 
 }  // namespace b200

@@ -973,8 +973,6 @@ GridShape grid_shape(int Np, int max_groups32, int max_groups64, int runners, in
     return {nb, groups, (tiles + groups - 1) / groups};
 }
 
-size_t align256(size_t bytes) { return (bytes + 255) & ~size_t(255); }
-
 }  // namespace
 
 // fp32 PyTorch layouts -> LstmLayerWeights: gate rows permuted by lstm_fused_row for lstm_size 96, W_ih's K padded to a
@@ -1003,14 +1001,19 @@ void free_lstm_layer(LstmLayerWeights& w) {
     w = LstmLayerWeights{};
 }
 
-size_t lstm_stack_workspace_bytes(int C, int num_layers, int T, int Np) {
-    if (C == FL_C) return 0;  // the fused layer computes gx in registers
-    const size_t gx = align256((size_t)T * Np * 4 * C * 2);
-    // lstm_grid_rec_kernel: at most one arrival counter per 32 chunks and layer, and the error word
-    return C > 384 ? gx + align256((size_t)num_layers * (Np / 32) * sizeof(unsigned int)) + 256 : gx;
+LstmStackBuffers carve_lstm_stack(Bump& b, int C, int num_layers, int T, int Np) {
+    LstmStackBuffers w;
+    if (C == FL_C) return w;  // the fused layer computes gx in registers
+    w.gx = b.take<__half>((size_t)T * Np * 4 * C * 2);
+    if (C > 384) {  // lstm_grid_rec_kernel: at most one arrival counter per 32 chunks and layer, and the error word
+        w.counter_bytes = (size_t)num_layers * (Np / 32) * sizeof(unsigned int);
+        w.counters = b.take<unsigned int>(w.counter_bytes);
+        w.error = b.take<int>(sizeof(int));
+    }
+    return w;
 }
 
-LstmStack::LstmStack(const LstmStackDesc& d, void* ws) : m_d(d) {
+LstmStack::LstmStack(const LstmStackDesc& d, const LstmStackBuffers& ws) : m_d(d), m_ws(ws) {
     const int C = d.C, Np = d.Np;
     if (const char* dbg = std::getenv("B200_DEBUG_LSTM_LAYERS")) m_debug_layers = std::atoi(dbg);
     if (C == FL_C) {  // one lstm_layer_kernel per layer
@@ -1018,13 +1021,6 @@ LstmStack::LstmStack(const LstmStackDesc& d, void* ws) : m_d(d) {
         m_groups = Np / FL_NB;
         return;
     }
-    uint8_t* base = static_cast<uint8_t*>(ws);
-    auto take = [&](size_t bytes) {
-        uint8_t* p = base;
-        base += align256(bytes);
-        return p;
-    };
-    m_gx = reinterpret_cast<__half*>(take((size_t)d.T * Np * 4 * C * 2));
     if (C <= 384) {  // one cluster per m_nb chunks, all in one launch
         m_kind = Kind::Rec;
         m_nb = lstm_rec_chunks(Np);
@@ -1049,9 +1045,6 @@ LstmStack::LstmStack(const LstmStackDesc& d, void* ws) : m_d(d) {
         m_groups = s.groups;
         m_launches = s.launches;
         m_group_ctas = C / GR_UNITS;
-        m_counter_bytes = (size_t)d.num_layers * (Np / 32) * sizeof(unsigned int);
-        m_counters = reinterpret_cast<unsigned int*>(take(m_counter_bytes));
-        m_error = reinterpret_cast<int*>(take(sizeof(int)));
     }
     // With three or more batches in flight the x-projection GEMMs keep off some SMs, so that another batch's recurrence
     // (several milliseconds of latency chain) can start beside them instead of queueing behind a GEMM that owns every SM.
@@ -1070,14 +1063,14 @@ LstmStack::LstmStack(const LstmStackDesc& d, void* ws) : m_d(d) {
         g.K = (C + 63) / 64 * 64;
         g.bias = w.bias;
         g.act = GEMM_ACT_NONE;
-        g.out = m_gx;
+        g.out = m_ws.gx;
         g.out_m1 = 1;
         g.out_s0 = 4 * C;
         g.max_ctas = gemm_cap;
         m_gx_gemm.push_back(make_gemm_plan(g));
     }
-    if (m_error) {
-        B200_CUDA(cudaMemset(m_error, 0, sizeof(int)));
+    if (m_ws.error) {
+        B200_CUDA(cudaMemset(m_ws.error, 0, sizeof(int)));
         B200_CUDA(cudaHostAlloc(&m_error_host, sizeof(int), cudaHostAllocDefault));
         *m_error_host = 0;
     }
@@ -1093,7 +1086,7 @@ bool LstmStack::run(cudaStream_t stream, ProfileSink* prof) {
         if (prof) prof->mark(name, stream);
     };
     const int C = m_d.C, Np = m_d.Np;
-    if (m_counters) B200_CUDA(cudaMemsetAsync(m_counters, 0, m_counter_bytes, stream));
+    if (m_ws.counters) B200_CUDA(cudaMemsetAsync(m_ws.counters, 0, m_ws.counter_bytes, stream));
     const int nl = m_debug_layers >= 0 && m_debug_layers < m_d.num_layers ? m_debug_layers : m_d.num_layers;
     for (int l = 0; l < nl; ++l) {
         NvtxRange r("lstm_layer");
@@ -1110,9 +1103,9 @@ bool LstmStack::run(cudaStream_t stream, ProfileSink* prof) {
         // launch i covers groups i * m_groups .. of m_nb chunks, with counters of its own (the last may hold fewer groups)
         for (int i = 0; i < m_launches; ++i) {
             const int ctas = std::min(m_groups, Np / m_nb - i * m_groups) * m_group_ctas;
-            unsigned int* counters = m_counters ? m_counters + (size_t)l * (Np / 32) + (size_t)i * m_groups : nullptr;
-            const LstmRecParams p{m_d.seq, m_gx, w.w_hh, m_d.T, Np, reverse, m_lens, m_d.stride, i * m_groups * m_nb,
-                                  counters, m_error};
+            unsigned int* counters = m_ws.counters ? m_ws.counters + (size_t)l * (Np / 32) + (size_t)i * m_groups : nullptr;
+            const LstmRecParams p{m_d.seq, m_ws.gx, w.w_hh, m_d.T, Np, reverse, m_lens, m_d.stride, i * m_groups * m_nb,
+                                  counters, m_ws.error};
             if (m_kind == Kind::Rec) {
                 launch_lstm_rec(C, m_nb, ctas, p, stream);
                 mark("lstm_rec");
@@ -1123,14 +1116,14 @@ bool LstmStack::run(cudaStream_t stream, ProfileSink* prof) {
         }
     }
     // the error word of the grid recurrence, read by check_errors() once the stream has drained
-    if (m_error_host) B200_CUDA(cudaMemcpyAsync(m_error_host, m_error, sizeof(int), cudaMemcpyDeviceToHost, stream));
+    if (m_error_host) B200_CUDA(cudaMemcpyAsync(m_error_host, m_ws.error, sizeof(int), cudaMemcpyDeviceToHost, stream));
     return nl == m_d.num_layers;
 }
 
 void LstmStack::check_errors() {
     if (!m_error_host || *m_error_host == 0) return;
     *m_error_host = 0;
-    B200_CUDA(cudaMemset(m_error, 0, sizeof(int)));
+    B200_CUDA(cudaMemset(m_ws.error, 0, sizeof(int)));
     throw std::runtime_error("lstm_grid_rec_kernel: a group of CTAs did not reach its step barrier within the time "
                              "budget; the outputs of this batch are invalid");
 }
@@ -1200,6 +1193,15 @@ public:
     int Cp = 0, out1 = 0, out1p = 0;
 
 private:
+    struct Buffers {
+        __half* x2;    // conv2 output [N][t_pad][16]: first, the tests read it at offset 0
+        __half* seq;   // [T_out + 1][Np][C]: second, the tests read it right behind x2
+        __half* mid;   // decomposition only: [T_out][Np][out_features]
+        int* tile_counter;  // conv12_tc_kernel
+        LstmStackBuffers lstm;
+    };
+    // The workspace layout for N chunks of T_in samples; refuses a batch the LSTM kernels cannot take
+    Buffers carve(Bump& b, int N, int T_in) const;
     int pad3() const { return desc.convs[2].winlen / 2; }
     int t_pad(int T_in) const { return T_in + 2 * pad3() + 8; }
     // lstm_size 96 keeps the reference's fixed-size contract (batch a multiple of 16, no variable chunk sizes); the larger
@@ -1314,17 +1316,7 @@ LstmModel::~LstmModel() {
     cudaFree(wl2);
 }
 
-size_t LstmModel::workspace_bytes(int N, int T_in) const {
-    const int T_out = T_in / desc.stride;
-    const size_t x2 = (size_t)N * t_pad(T_in) * 16 * 2 + 4096;
-    const size_t seq = (size_t)(T_out + 1) * n_pad(N) * desc.lstm_size * 2 + 4096;
-    const size_t mid = desc.out_features > 0 ? (size_t)T_out * n_pad(N) * desc.out_features * 2 + 4096 : 0;
-    const size_t lstm = lstm_stack_workspace_bytes(desc.lstm_size, desc.lstm_layers, T_out, n_pad(N));
-    return x2 + seq + mid + lstm + 4096;  // + the tile counter of conv12_tc_kernel
-}
-
-std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half* signal, __half* scores, void* ws,
-                                                  size_t ws_bytes) {
+LstmModel::Buffers LstmModel::carve(Bump& b, int N, int T_in) const {
     const int C = desc.lstm_size;
     const int T_out = T_in / desc.stride;
     const int Np = n_pad(N);
@@ -1333,20 +1325,31 @@ std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half*
         throw std::invalid_argument(large() ? "batch_size must be a multiple of 32 for this LSTM size"
                                               : "batch_size must be a multiple of 16 for LSTM models");
     }
+    Buffers w;
+    w.x2 = b.take<__half>((size_t)N * t_pad(T_in) * 16 * 2);
+    w.seq = b.take<__half>((size_t)(T_out + 1) * Np * C * 2);
+    w.mid = desc.out_features > 0 ? b.take<__half>((size_t)T_out * Np * desc.out_features * 2) : nullptr;
+    w.tile_counter = b.take<int>(sizeof(int));
+    w.lstm = carve_lstm_stack(b, C, desc.lstm_layers, T_out, Np);
+    return w;
+}
+
+size_t LstmModel::workspace_bytes(int N, int T_in) const {
+    Bump sizing;
+    carve(sizing, N, T_in);
+    return sizing.used();
+}
+
+std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half* signal, __half* scores, void* ws,
+                                                  size_t ws_bytes) {
+    const int C = desc.lstm_size;
+    const int T_out = T_in / desc.stride;
+    const int Np = n_pad(N);
+    Bump b(ws, ws_bytes);
+    const auto [x2, seq, mid, tile_counter, lstm_ws] = carve(b, N, T_in);
+    if (b.used() != ws_bytes) throw std::logic_error("LSTM workspace: the plan's layout differs from workspace_bytes()");
     auto plan = std::make_unique<LstmPlan>();
-    uint8_t* base = static_cast<uint8_t*>(ws);
-    auto take = [&](size_t bytes) {
-        uint8_t* p = base;
-        base += (bytes + 255) & ~size_t(255);
-        if ((size_t)(base - static_cast<uint8_t*>(ws)) > ws_bytes) throw std::logic_error("LSTM workspace overflow");
-        return p;
-    };
     const int Tp = t_pad(T_in);
-    __half* x2 = reinterpret_cast<__half*>(take((size_t)N * Tp * 16 * 2));
-    __half* seq = reinterpret_cast<__half*>(take((size_t)(T_out + 1) * Np * C * 2));
-    __half* mid = desc.out_features > 0 ? reinterpret_cast<__half*>(take((size_t)T_out * Np * desc.out_features * 2)) : nullptr;
-    int* tile_counter = reinterpret_cast<int*>(take(256));
-    void* lstm_ws = take(lstm_stack_workspace_bytes(C, desc.lstm_layers, T_out, Np));
 
     // conv1 + conv2
     plan->conv12 = Conv12Params{signal, x2, conv_w, N, T_in, Tp, pad3(), desc.convs[0].size, desc.convs[0].winlen,
@@ -1364,7 +1367,6 @@ std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half*
 
     // conv3: rows (n, t) read K3p contiguous halfs starting at x2[n][stride * t]
     {
-        if (T_in % desc.stride != 0) throw std::invalid_argument("chunk size must be a multiple of the model stride");
         GemmDesc g{};
         g.a = x2;
         g.batches = N;

@@ -387,26 +387,21 @@ void ModBaseRunner::init() {
     const int Tp_seq = e.seq_len + 2 * (q2.winlen / 2) + K2 / 16;
     const int Cm = mc.insize;
     const int Tp_m = e.t_enc + 2 * (mc.winlen / 2) + Km / Cm + 1;
-    const size_t seq_b = (size_t)(T + 1) * N * C * 2, x2_b = (size_t)N * Tp_sig * 16 * 2, y1_b = (size_t)N * Tp_seq * 16 * 2,
-                 m_b = (size_t)N * Tp_m * Cm * 2, lstm_b = lstm_stack_workspace_bytes(C, 2, T, N);
-    auto al = [](size_t b) { return (b + 255) & ~size_t(255); };
-    m_ws_bytes = al(seq_b) + al(x2_b) + al(y1_b) + al(m_b) + lstm_b;
-    m_arena.reserve(al(sig_b) + al(kmer_b) + al(out_b) + m_ws_bytes);
-    m_d_ws = m_arena.take(m_ws_bytes);
-    uint8_t* base = static_cast<uint8_t*>(m_d_ws);
-    auto take = [&](size_t b) {
-        uint8_t* p = base;
-        base += al(b);
-        return p;
-    };
-    __half* seq = reinterpret_cast<__half*>(take(seq_b));  // first: tests read it at offset 0
-    __half* x2 = reinterpret_cast<__half*>(take(x2_b));
-    __half* y1 = reinterpret_cast<__half*>(take(y1_b));
-    __half* merge_in = reinterpret_cast<__half*>(take(m_b));
-    void* lstm_ws = take(lstm_b);
-    m_d_sig = static_cast<__half*>(m_arena.take(sig_b));
-    m_d_kmers = static_cast<int8_t*>(m_arena.take(kmer_b));
-    m_d_out = static_cast<__half*>(m_arena.take(out_b));
+    __half *seq = nullptr, *x2 = nullptr, *y1 = nullptr, *merge_in = nullptr;
+    LstmStackBuffers lstm_ws;
+    m_arena.allocate([&](Bump& b) {
+        // the workspace: everything up to the input and output buffers
+        seq = b.take<__half>((size_t)(T + 1) * N * C * 2);  // first: tests read it at offset 0
+        x2 = b.take<__half>((size_t)N * Tp_sig * 16 * 2);
+        y1 = b.take<__half>((size_t)N * Tp_seq * 16 * 2);
+        merge_in = b.take<__half>((size_t)N * Tp_m * Cm * 2);
+        lstm_ws = carve_lstm_stack(b, C, 2, T, N);
+        m_ws_bytes = b.used();
+        m_d_sig = b.take<__half>(sig_b);
+        m_d_kmers = b.take<int8_t>(kmer_b);
+        m_d_out = b.take<__half>(out_b);
+    });
+    m_d_ws = seq;
     // padding rows stay zero: the kernels write interior rows only
     B200_CUDA(cudaMemsetAsync(m_d_ws, 0, m_ws_bytes, m_stream));
     B200_CUDA(cudaMemsetAsync(m_d_sig, 0, sig_b, m_stream));

@@ -407,6 +407,13 @@ private:
         std::vector<int> pad;    // front padding of that buffer (= next conv's winlen/2)
     };
     Shapes shapes(int T_in) const;
+    struct Buffers {
+        std::vector<__half*> cbuf;  // output of conv i (but the last), [N][t_pad[i]][size]
+        __half *x, *y, *att, *qkv, *hid, *ups;
+        float *ss_a, *ss_b;  // partial sums of squares (folded RMSNorm) of the rows in x and in y
+    };
+    // The workspace layout for N chunks of T_in samples; refuses a chunk longer than the RoPE table
+    Buffers carve(Bump& b, int N, int T_in) const;
 };
 
 TxModel::Shapes TxModel::shapes(int T_in) const {
@@ -568,49 +575,43 @@ TxModel::~TxModel() {
     for (void* p : owned) cudaFree(p);
 }
 
-size_t TxModel::workspace_bytes(int N, int T_in) const {
+TxModel::Buffers TxModel::carve(Bump& b, int N, int T_in) const {
     const Shapes s = shapes(T_in);
-    size_t total = 0;
-    auto al = [](size_t b) { return (b + 255) & ~size_t(255); };
-    for (int i = 0; i + 1 < desc.num_convs; ++i) total += al((size_t)N * s.t_pad[i] * desc.convs[i].size * 2);
-    const size_t rows = (size_t)N * s.t.back();
-    const size_t dm = (size_t)desc.d_model;
-    total += al(rows * dm * 2) * 3;                                 // x, y, attn out
-    total += al(rows * 3 * dm * 2);                                 // qkv
-    total += al(rows * (size_t)desc.dim_feedforward * 2);           // ff hidden
-    total += al(rows * (size_t)desc.upsample_scale * dm * 2);       // upsampled
-    total += al(rows * (size_t)gemm_out_ss_parts((int)dm) * 4) * 2;   // partial sums of squares (folded RMSNorm), two in flight
-    return total + 4096;
+    const int T = s.t.back();
+    if (T > (desc.max_seq_len > 0 ? desc.max_seq_len : 2048)) {
+        throw std::invalid_argument("RotE - maximum sequence length exceeded - your chunksize may be too large");
+    }
+    Buffers w;
+    for (int i = 0; i + 1 < desc.num_convs; ++i) w.cbuf.push_back(b.take<__half>((size_t)N * s.t_pad[i] * desc.convs[i].size * 2));
+    const size_t rows = (size_t)N * T, dm = desc.d_model;
+    w.x = b.take<__half>(rows * dm * 2);
+    w.y = b.take<__half>(rows * dm * 2);
+    w.att = b.take<__half>(rows * dm * 2);
+    w.qkv = b.take<__half>(rows * 3 * dm * 2);
+    w.hid = b.take<__half>(rows * desc.dim_feedforward * 2);
+    w.ups = b.take<__half>(rows * desc.upsample_scale * dm * 2);
+    w.ss_a = b.take<float>(rows * gemm_out_ss_parts((int)dm) * 4);   // x: after fc2 / the previous layer
+    w.ss_b = b.take<float>(rows * gemm_out_ss_parts((int)dm) * 4);   // y: after out_proj
+    return w;
+}
+
+size_t TxModel::workspace_bytes(int N, int T_in) const {
+    Bump sizing;
+    carve(sizing, N, T_in);
+    return sizing.used();
 }
 
 std::unique_ptr<ForwardPlan> TxModel::make_plan(int N, int T_in, const __half* signal, __half* scores, void* ws,
                                                 size_t ws_bytes) {
     const Shapes s = shapes(T_in);
     const int T = s.t.back();
-    if (T > (desc.max_seq_len > 0 ? desc.max_seq_len : 2048)) {
-        throw std::invalid_argument("RotE - maximum sequence length exceeded - your chunksize may be too large");
-    }
+    Bump b(ws, ws_bytes);
+    const auto [cbuf, x, y, att, qkv, hid, ups, ss_a, ss_b] = carve(b, N, T_in);
+    if (b.used() != ws_bytes) throw std::logic_error("tx workspace: the plan's layout differs from workspace_bytes()");
     auto plan = std::make_unique<TxPlan>();
-    uint8_t* base = static_cast<uint8_t*>(ws);
-    auto take = [&](size_t bytes) {
-        uint8_t* p = base;
-        base += (bytes + 255) & ~size_t(255);
-        if ((size_t)(base - static_cast<uint8_t*>(ws)) > ws_bytes) throw std::logic_error("tx workspace overflow");
-        return reinterpret_cast<__half*>(p);
-    };
-    std::vector<__half*> cbuf;
-    for (int i = 0; i + 1 < desc.num_convs; ++i) cbuf.push_back(take((size_t)N * s.t_pad[i] * desc.convs[i].size * 2));
     const long long rows = (long long)N * T;
     const int dm = desc.d_model, dqkv = 3 * desc.d_model;
-    __half* x = take((size_t)rows * dm * 2);
-    __half* y = take((size_t)rows * dm * 2);
-    __half* att = take((size_t)rows * dm * 2);
-    __half* qkv = take((size_t)rows * dqkv * 2);
-    __half* hid = take((size_t)rows * desc.dim_feedforward * 2);
-    __half* ups = take((size_t)rows * desc.upsample_scale * dm * 2);
     const int ssp = gemm_out_ss_parts(dm);
-    float* ss_a = reinterpret_cast<float*>(take((size_t)rows * ssp * 4));   // of the rows in x (after fc2 / the previous layer)
-    float* ss_b = reinterpret_cast<float*>(take((size_t)rows * ssp * 4));   // of the rows in y (after out_proj)
 
     plan->conv1 = Conv1Params{signal, cbuf[0], conv1_w, N, T_in, s.t_pad[0], s.pad[0], desc.convs[0].size, desc.convs[0].winlen,
                               desc.convs[0].activation};
@@ -877,10 +878,12 @@ void test_attention_host(int device, const uint16_t* qkv, int N, int T, int H, i
     check_attention_window(win_upper, win_lower);
     require_sm90(device);
     const size_t rows = (size_t)N * T, qkv_b = rows * 3 * H * ATT_D * 2, out_b = rows * H * ATT_D * 2;
+    __half *d_qkv = nullptr, *d_out = nullptr;
     Arena arena;
-    arena.reserve(qkv_b + out_b + 4096);
-    auto* d_qkv = static_cast<__half*>(arena.take(qkv_b));
-    auto* d_out = static_cast<__half*>(arena.take(out_b));
+    arena.allocate([&](Bump& b) {
+        d_qkv = b.take<__half>(qkv_b);
+        d_out = b.take<__half>(out_b);
+    });
     B200_CUDA(cudaMemcpy(d_qkv, qkv, qkv_b, cudaMemcpyHostToDevice));
     B200_CUDA(cudaMemset(d_out, 0, out_b));
     const CUtensorMap map = make_tmap_2d(d_qkv, (uint64_t)3 * H * ATT_D, (uint64_t)rows, (uint64_t)3 * H * ATT_D * 2, ATT_D, AT_BQ);

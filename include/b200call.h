@@ -285,7 +285,8 @@ B200_API int b200_stitch_chunks(const b200_called_chunk* chunks,
 /* ---- Batch-size selection (SURVEY.md 8f row 4; CudaCaller::determine_batch_dims, CudaCaller.cpp:372-632) --------
  *
  * Device bytes one runner of (batch_size, chunk_size) allocates: exact, from the launch plan.  (The reference estimates
- * it from per-model tables of bytes per chunk-timestep, CudaCaller::calculate_memory_requirements, :323-370.) */
+ * it from per-model tables of bytes per chunk-timestep, CudaCaller::calculate_memory_requirements, :323-370.)  Returns
+ * B200_ERR_INVALID for every shape b200_runner_create refuses. */
 B200_API int b200_engine_runner_bytes(b200_engine* engine, int32_t batch_size, int32_t chunk_size, uint64_t* bytes);
 /* The benchmark loop of determine_batch_dims (:530-557): for batch sizes granularity, 2*granularity, ... <=
  * max_batch_size, run the path twice on a scratch runner and keep the smaller time per chunk.  The reference times
