@@ -7,13 +7,33 @@
 #include "engine.h"
 
 #include <cmath>
+#include <cstddef>
 #include <cstring>
 #include <limits>
 #include <string>
 
+// the exported symbols of these names serve binaries built against earlier headers (b200call.h)
+#undef b200_engine_create
+#undef b200_pool_create
+
 namespace {
 
 thread_local std::string g_last_error;
+
+// What a binary built against a header without lstm_precision passes: the fields up to and including tx_precision
+constexpr size_t kDescSizeBeforeLstmPrecision = offsetof(b200_model_desc, lstm_precision);
+
+// The caller's descriptor of desc_size bytes as this library's: fields the caller's header does not have are zero
+b200_model_desc read_desc(const b200_model_desc* desc, size_t desc_size) {
+    if (desc_size < kDescSizeBeforeLstmPrecision) throw std::invalid_argument("b200_model_desc: desc_size is smaller than any published descriptor");
+    const unsigned char* bytes = reinterpret_cast<const unsigned char*>(desc);
+    for (size_t i = sizeof(b200_model_desc); i < desc_size; ++i) {
+        if (bytes[i] != 0) throw b200::Unsupported("b200_model_desc: the descriptor sets fields this library does not know");
+    }
+    b200_model_desc d{};
+    std::memcpy(&d, desc, desc_size < sizeof(d) ? desc_size : sizeof(d));
+    return d;
+}
 
 template <typename F>
 int guarded(F&& fn) {
@@ -62,12 +82,17 @@ void b200_default_decoder_options(b200_decoder_options* o) {
     o->move_pad = 0;
 }
 
-int b200_engine_create(const b200_model_desc* desc, const b200_tensor* tensors, int32_t num_tensors, int32_t device,
-                       b200_engine** out) {
+int b200_engine_create_sized(const b200_model_desc* desc, size_t desc_size, const b200_tensor* tensors, int32_t num_tensors,
+                             int32_t device, b200_engine** out) {
     return guarded([&] {
         if (!desc || !tensors || !out) throw std::invalid_argument("b200_engine_create: null argument");
-        *out = reinterpret_cast<b200_engine*>(new b200::Engine(*desc, tensors, num_tensors, device));
+        *out = reinterpret_cast<b200_engine*>(new b200::Engine(read_desc(desc, desc_size), tensors, num_tensors, device));
     });
+}
+
+int b200_engine_create(const b200_model_desc* desc, const b200_tensor* tensors, int32_t num_tensors, int32_t device,
+                       b200_engine** out) {
+    return b200_engine_create_sized(desc, kDescSizeBeforeLstmPrecision, tensors, num_tensors, device, out);
 }
 
 int b200_engine_destroy(b200_engine* e) {
@@ -140,13 +165,20 @@ int b200_engine_batch_timeouts_ms(const b200_engine* e, int32_t* first_chunk_ms,
     });
 }
 
-int b200_pool_create(const b200_model_desc* desc, const b200_tensor* tensors, int32_t num_tensors, const int32_t* devices,
-                     int32_t num_devices, int32_t runners_per_device, int32_t batch_size, int32_t chunk_size, b200_pool** out) {
+int b200_pool_create_sized(const b200_model_desc* desc, size_t desc_size, const b200_tensor* tensors, int32_t num_tensors,
+                           const int32_t* devices, int32_t num_devices, int32_t runners_per_device, int32_t batch_size,
+                           int32_t chunk_size, b200_pool** out) {
     return guarded([&] {
         if (!desc || !tensors || !devices || !out) throw std::invalid_argument("b200_pool_create: null argument");
-        *out = reinterpret_cast<b200_pool*>(
-                new b200::Pool(*desc, tensors, num_tensors, devices, num_devices, runners_per_device, batch_size, chunk_size));
+        *out = reinterpret_cast<b200_pool*>(new b200::Pool(read_desc(desc, desc_size), tensors, num_tensors, devices, num_devices,
+                                                           runners_per_device, batch_size, chunk_size));
     });
+}
+
+int b200_pool_create(const b200_model_desc* desc, const b200_tensor* tensors, int32_t num_tensors, const int32_t* devices,
+                     int32_t num_devices, int32_t runners_per_device, int32_t batch_size, int32_t chunk_size, b200_pool** out) {
+    return b200_pool_create_sized(desc, kDescSizeBeforeLstmPrecision, tensors, num_tensors, devices, num_devices,
+                                  runners_per_device, batch_size, chunk_size, out);
 }
 
 int b200_pool_destroy(b200_pool* p) {
@@ -379,6 +411,21 @@ int b200_test_gemm_fp8(int32_t device, const uint8_t* a, const uint8_t* b, int32
     return guarded([&] {
         if (!a || !b || !c) throw std::invalid_argument("b200_test_gemm_fp8: null argument");
         b200::test_gemm_fp8_host(device, a, b, M, N, K, activation, residual, alpha, c);
+    });
+}
+
+int b200_test_gemm_s8(int32_t device, const int8_t* a, const int8_t* b, const float* col_scale, const float* bias, int32_t M,
+                      int32_t N, int32_t K, int32_t activation, uint16_t* c) {
+    return guarded([&] {
+        if (!a || !b || !col_scale || !c) throw std::invalid_argument("b200_test_gemm_s8: null argument");
+        b200::test_gemm_s8_host(device, a, b, col_scale, bias, M, N, K, activation, c);
+    });
+}
+
+int b200_test_quantize_rows(const uint16_t* f16, int32_t rows, int32_t cols, int8_t* q, uint16_t* scale) {
+    return guarded([&] {
+        if (rows < 1 || cols < 1 || !f16 || !q || !scale) throw std::invalid_argument("b200_test_quantize_rows: bad argument");
+        b200::quantize_rows_f16(f16, rows, cols, q, scale);
     });
 }
 

@@ -91,6 +91,12 @@ Engine::Engine(const b200_model_desc& desc, const b200_tensor* tensors, int num_
     if (desc.tx_precision == B200_TX_FP8_FFN && desc.model_type != B200_MODEL_TX) {
         throw std::invalid_argument("the fp8_ffn precision applies to transformer models only; LSTM models run in fp16");
     }
+    if (desc.lstm_precision != B200_LSTM_FP16 && desc.lstm_precision != B200_LSTM_INT8) {
+        throw std::invalid_argument("lstm_precision must be B200_LSTM_FP16 (0) or B200_LSTM_INT8 (1)");
+    }
+    if (desc.lstm_precision == B200_LSTM_INT8 && desc.model_type != B200_MODEL_LSTM) {
+        throw std::invalid_argument("the int8_lstm precision applies to LSTM models only; transformer models have fp8_ffn");
+    }
     require_sm90(device);
     B200_CUDA(cudaStreamCreateWithFlags(&m_stream, cudaStreamNonBlocking));
     if (desc.model_type == B200_MODEL_LSTM) {

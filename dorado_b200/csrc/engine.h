@@ -378,6 +378,13 @@ void test_attention_host(int device, const uint16_t* qkv, int N, int T, int H, i
 void test_gemm_fp8_host(int device, const uint8_t* a, const uint8_t* b, int M, int N, int K, int activation,
                         const uint16_t* residual, float alpha, void* c);
 
+void test_gemm_s8_host(int device, const int8_t* a, const int8_t* b, const float* col_scale, const float* bias, int M, int N,
+                       int K, int activation, uint16_t* c);
+// Host quantisation of the int8_lstm weights (lstm_model.cu): utils::quantize_tensor(w, 1) on fp16 bits [rows][cols] ->
+// int8 and the fp16 scale of every row; and the fp32 factor 1 / (kInt8ActScale * scale) a row's accumulator is multiplied by
+void quantize_rows_f16(const uint16_t* w16, int rows, int cols, int8_t* q, uint16_t* scale16);
+float int8_row_inv(uint16_t scale16);
+
 // Host rounding of the fp8_ffn weights (tx_model.cu): fp16 bits of a float (round to nearest even), the reference's
 // remove_bits on fp16 bits, fp16(v) with remove_bits as float, and torch's float8_e4m3fn cast of an fp16 value.
 uint16_t f16_bits(float v);

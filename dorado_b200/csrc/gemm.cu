@@ -10,6 +10,9 @@
 // and run the epilogue (bias / activation / residual / rotary / SwiGLU -> fp16 -> global) from the accumulator fragments.
 // E4M3 form (template FP8, the transformer's fc1 / fc2 in the fp8_ffn precision): the same ring, tiles and epilogues with
 // 128 E4M3 per 128-byte K row instead of 64 fp16, wgmma m64n32k32.e4m3 and the SwiGLU output cast to E4M3.
+// int8 form (template Q8 = GEMM_Q8_OPERANDS, the x-projection and the CRF linear of LSTM models in the int8_lstm precision):
+// the E4M3 form's ring and boxes, wgmma m64n32k32.s8 into s32 accumulators, which the epilogue converts and multiplies by a
+// per-column fp32 factor.  Q8 = GEMM_Q8_STORE is the fp16 form whose tanh epilogue stores int8 (those models' last conv).
 // A is addressed through a 3-D tensor map (k, row, batch) so that overlapping-row views work: the last conv of the LSTM
 // models reads its im2col rows straight from the NTC activation buffer with row stride = stride * C_in (the reference's
 // "cutlass_conv" trick, ConvStack.cpp:236-275).
@@ -20,6 +23,7 @@
 
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 #include <vector>
 
 namespace b200 {
@@ -56,6 +60,7 @@ struct GemmKernelParams {
     const float* res_gain;
     int a_ss_parts, res_ss_parts;
     float norm_inv_dim, norm_eps;
+    const float* col_scale;   // GEMM_Q8_OPERANDS
 };
 
 // i-th tile of this CTA: row tile mt, column tile nt; false when the CTA has run out of tiles.  Producer and consumers walk
@@ -86,13 +91,15 @@ __device__ __forceinline__ float act_apply(float v) {
 
 // One K block (128 bytes: 64 fp16 or 128 E4M3) of a warpgroup's 64 x 32 NCH tile: 32 rows of W are 4 KB further on,
 // 32 bytes along K (16 fp16, 32 E4M3: one wgmma) are +2 in the (addr >> 4) field of a descriptor.
-template <int NCH, bool FP8>
-__device__ __forceinline__ void wgmma_k_block(float (&acc)[BN_MAX / 32][16], uint64_t adesc, uint64_t bdesc, bool accumulate) {
+template <int NCH, bool FP8, typename Acc>
+__device__ __forceinline__ void wgmma_k_block(Acc (&acc)[BN_MAX / 32][16], uint64_t adesc, uint64_t bdesc, bool accumulate) {
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
 #pragma unroll
         for (int c = 0; c < NCH; ++c) {
-            if constexpr (FP8) {
+            if constexpr (std::is_same_v<Acc, int32_t>) {
+                tc::wgmma_m64n32k32_s8(acc[c], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(c * 256 + 2 * k), accumulate || k != 0);
+            } else if constexpr (FP8) {
                 tc::wgmma_m64n32k32_e4m3(acc[c], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(c * 256 + 2 * k), accumulate || k != 0);
             } else {
                 tc::wgmma_m64n32k16(acc[c], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(c * 256 + 2 * k), accumulate || k != 0);
@@ -101,11 +108,13 @@ __device__ __forceinline__ void wgmma_k_block(float (&acc)[BN_MAX / 32][16], uin
     }
 }
 
-template <int ACT, bool FP8>
+template <int ACT, bool FP8, int Q8 = GEMM_Q8_NONE>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a,
                                                                      const __grid_constant__ CUtensorMap tma_w,
                                                                      const GemmKernelParams p) {
-    constexpr int KB = FP8 ? BK8 : BK;   // K elements per block
+    constexpr bool S8 = Q8 == GEMM_Q8_OPERANDS;
+    constexpr int KB = FP8 || S8 ? BK8 : BK;   // K elements per block
+    using Acc = std::conditional_t<S8, int32_t, float>;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // realign by an integer offset from the __shared__ symbol so the compiler keeps the shared address space
     uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -161,7 +170,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
     uint32_t ph = 0;
     int mt, nt;
     for (int ti = 0; gemm_tile_at(p, ti, &mt, &nt); ++ti) {
-        float acc[BN_MAX / 32][16];
+        Acc acc[BN_MAX / 32][16];
         int prev = -1;   // stage read by the wgmma group still in flight
         for (int kb = 0; kb < p.num_k_blocks; ++kb) {
             tc::mbar_wait_silent(&full[s], ph);
@@ -219,7 +228,27 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
             }
             row_bias[h] = (p.bias && p.bias_per_row && valid[h]) ? __ldg(p.bias + g[h]) : 0.0f;
         }
-        if constexpr (ACT == GEMM_ACT_ROPE) {
+        if constexpr (S8) {
+            // s32 -> fp32 is exact for the K this form is used at (|acc| <= 127^2 K < 2^24 up to K = 1024)
+#pragma unroll
+            for (int c = 0; c < BN_MAX / 32; ++c) {
+                if (c >= nch) continue;
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int nc = n0 + c * 32 + 8 * j + 2 * quad;
+                    const float2 sc = __ldg(reinterpret_cast<const float2*>(p.col_scale + nc));
+                    float2 b2 = make_float2(0.0f, 0.0f);
+                    if (p.bias) b2 = __ldg(reinterpret_cast<const float2*>(p.bias + nc));
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        if (!valid[h]) continue;
+                        const float v0 = fmaf((float)acc[c][4 * j + 2 * h], sc.x, b2.x);
+                        const float v1 = fmaf((float)acc[c][4 * j + 2 * h + 1], sc.y, b2.y);
+                        *reinterpret_cast<__half2*>(p.out + off[h] + nc) = __floats2half2_rn(act_apply<ACT>(v0), act_apply<ACT>(v1));
+                    }
+                }
+            }
+        } else if constexpr (ACT == GEMM_ACT_ROPE) {
             // head_dim 64 = two 32-column chunks (x1 | x2): out1 = cos*x1 - sin*x2, out2 = sin*x1 + cos*x2
 #pragma unroll
             for (int c = 0; c < BN_MAX / 32; c += 2) {
@@ -289,7 +318,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                                 ss_out[h][c] = fmaf(f.x, f.x, ss_out[h][c]);
                                 ss_out[h][c] = fmaf(f.y, f.y, ss_out[h][c]);
                             }
-                            *reinterpret_cast<__half2*>(p.out + off[h] + coff) = o;
+                            if constexpr (Q8 == GEMM_Q8_STORE) {
+                                const int32_t q0 = tc::cvt_rni_sat_s8(kInt8ActScale * act_apply<ACT>(v0));
+                                const int32_t q1 = tc::cvt_rni_sat_s8(kInt8ActScale * act_apply<ACT>(v1));
+                                *reinterpret_cast<uint16_t*>(reinterpret_cast<int8_t*>(p.out) + off[h] + coff) =
+                                        (uint16_t)((q0 & 0xff) | ((q1 & 0xff) << 8));
+                            } else {
+                                *reinterpret_cast<__half2*>(p.out + off[h] + coff) = o;
+                            }
                         }
                     }
                 }
@@ -380,10 +416,21 @@ int gemm_out_ss_parts(int N) {
 }
 
 GemmPlan make_gemm_plan(const GemmDesc& d) {
-    const int kb = d.fp8 ? BK8 : BK;
-    const int eb = d.fp8 ? 1 : 2;   // bytes per A / W element
+    const bool s8 = d.q8 == GEMM_Q8_OPERANDS;
+    const int kb = d.fp8 || s8 ? BK8 : BK;
+    const int eb = d.fp8 || s8 ? 1 : 2;   // bytes per A / W element
     if (d.K % kb != 0 || d.K <= 0) {
-        throw std::invalid_argument(d.fp8 ? "gemm: E4M3 K must be a positive multiple of 128" : "gemm: K must be a positive multiple of 64");
+        throw std::invalid_argument(eb == 1 ? "gemm: E4M3 / int8 K must be a positive multiple of 128" : "gemm: K must be a positive multiple of 64");
+    }
+    if (d.q8 != GEMM_Q8_NONE) {
+        const bool plain = !d.fp8 && !d.residual && !d.out_ss && !d.a_ss && !d.res_ss && !d.bias_per_row && d.out_col_m1 == 0;
+        if (s8 && !(plain && d.col_scale && (d.act == GEMM_ACT_NONE || d.act == GEMM_ACT_TANH_X5))) {
+            throw std::invalid_argument("gemm: int8 operands take col_scale, a column bias and the plain or TANH_X5 epilogue only");
+        }
+        if (d.q8 == GEMM_Q8_STORE && !(plain && d.act == GEMM_ACT_TANH)) {
+            throw std::invalid_argument("gemm: the int8 store goes with fp16 operands and the TANH epilogue only");
+        }
+        if (!s8 && d.q8 != GEMM_Q8_STORE) throw std::invalid_argument("gemm: unknown q8 form");
     }
     if (d.fp8 && (d.act != GEMM_ACT_NONE && d.act != GEMM_ACT_SWIGLU)) {
         throw std::invalid_argument("gemm: E4M3 operands take the plain and SwiGLU epilogues only");
@@ -428,11 +475,11 @@ GemmPlan make_gemm_plan(const GemmDesc& d) {
     return p;
 }
 
-template <int ACT, bool FP8 = false>
+template <int ACT, bool FP8 = false, int Q8 = GEMM_Q8_NONE>
 static void launch_gemm(int grid, size_t smem, cudaStream_t stream, const CUtensorMap& a, const CUtensorMap& w,
                         const GemmKernelParams& k) {
-    ensure_dynamic_smem(gemm_wgmma_kernel<ACT, FP8>, 227 * 1024);
-    gemm_wgmma_kernel<ACT, FP8><<<grid, GEMM_THREADS, smem, stream>>>(a, w, k);
+    ensure_dynamic_smem(gemm_wgmma_kernel<ACT, FP8, Q8>, 227 * 1024);
+    gemm_wgmma_kernel<ACT, FP8, Q8><<<grid, GEMM_THREADS, smem, stream>>>(a, w, k);
 }
 
 void run_gemm(const GemmPlan& p, cudaStream_t stream) {
@@ -440,7 +487,7 @@ void run_gemm(const GemmPlan& p, cudaStream_t stream) {
     k.rows_per_batch = p.d.rows_per_batch;
     k.tiles_per_batch = p.tiles_per_batch;
     k.N = p.d.N;
-    k.num_k_blocks = p.d.K / (p.d.fp8 ? BK8 : BK);
+    k.num_k_blocks = p.d.K / (p.d.fp8 || p.d.q8 == GEMM_Q8_OPERANDS ? BK8 : BK);
     k.bn = p.bn;
     k.bias = p.d.bias;
     k.out = static_cast<__half*>(p.d.out);
@@ -468,11 +515,19 @@ void run_gemm(const GemmPlan& p, cudaStream_t stream) {
     k.res_ss_parts = p.d.res_ss_parts;
     k.norm_inv_dim = p.d.norm_dim > 0 ? 1.0f / (float)p.d.norm_dim : 0.0f;
     k.norm_eps = p.d.norm_eps;
+    k.col_scale = p.d.col_scale;
     const int max_ctas = p.d.max_ctas > 0 && p.d.max_ctas < kNumSMs ? p.d.max_ctas : kNumSMs;
     const int grid = k.num_tiles < max_ctas ? k.num_tiles : max_ctas;
     if (p.d.fp8) {
         if (p.d.act == GEMM_ACT_SWIGLU) launch_gemm<GEMM_ACT_SWIGLU, true>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
         else launch_gemm<GEMM_ACT_NONE, true>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
+        B200_CUDA(cudaGetLastError());
+        return;
+    }
+    if (p.d.q8 != GEMM_Q8_NONE) {
+        if (p.d.q8 == GEMM_Q8_STORE) launch_gemm<GEMM_ACT_TANH, false, GEMM_Q8_STORE>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
+        else if (p.d.act == GEMM_ACT_TANH_X5) launch_gemm<GEMM_ACT_TANH_X5, false, GEMM_Q8_OPERANDS>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
+        else launch_gemm<GEMM_ACT_NONE, false, GEMM_Q8_OPERANDS>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
         B200_CUDA(cudaGetLastError());
         return;
     }
@@ -580,6 +635,52 @@ void test_gemm_fp8_host(int device, const uint8_t* a, const uint8_t* b, int M, i
     run_gemm(plan, nullptr);
     B200_CUDA(cudaDeviceSynchronize());
     B200_CUDA(cudaMemcpy(c, d_c, out_bytes, cudaMemcpyDeviceToHost));
+}
+
+// int8 operands (A [M][K], W [N][K], K zero-padded to a multiple of 128): c = act(float(A W^T) * col_scale[n] + bias[n]), fp16
+void test_gemm_s8_host(int device, const int8_t* a, const int8_t* b, const float* col_scale, const float* bias, int M, int N,
+                       int K, int activation, uint16_t* c) {
+    if (M < 1 || N < 1 || K < 1) throw std::invalid_argument("test_gemm_s8: empty operand");
+    require_sm90(device);
+    const int Kp = (K + BK8 - 1) / BK8 * BK8;
+    int8_t *d_a = nullptr, *d_w = nullptr;
+    float *d_scale = nullptr, *d_bias = nullptr;
+    __half* d_c = nullptr;
+    Arena arena;
+    arena.allocate([&](Bump& bump) {
+        d_a = bump.take<int8_t>((size_t)M * Kp);
+        d_w = bump.take<int8_t>((size_t)N * Kp);
+        d_scale = bump.take<float>((size_t)N * 4);
+        d_bias = bump.take<float>((size_t)N * 4);
+        d_c = bump.take<__half>((size_t)M * N * 2);
+    });
+    B200_CUDA(cudaMemset(d_a, 0, (size_t)M * Kp));
+    B200_CUDA(cudaMemset(d_w, 0, (size_t)N * Kp));
+    B200_CUDA(cudaMemcpy2D(d_a, (size_t)Kp, a, (size_t)K, (size_t)K, M, cudaMemcpyHostToDevice));
+    B200_CUDA(cudaMemcpy2D(d_w, (size_t)Kp, b, (size_t)K, (size_t)K, N, cudaMemcpyHostToDevice));
+    B200_CUDA(cudaMemcpy(d_scale, col_scale, (size_t)N * 4, cudaMemcpyHostToDevice));
+    if (bias) B200_CUDA(cudaMemcpy(d_bias, bias, (size_t)N * 4, cudaMemcpyHostToDevice));
+    GemmDesc d{};
+    d.q8 = GEMM_Q8_OPERANDS;
+    d.col_scale = d_scale;
+    d.a = d_a;
+    d.batches = 1;
+    d.rows_per_batch = M;
+    d.a_row_stride = Kp;
+    d.a_batch_stride = (int64_t)M * Kp;
+    d.w = d_w;
+    d.N = N;
+    d.K = Kp;
+    d.bias = bias ? d_bias : nullptr;
+    d.act = activation;
+    d.out = d_c;
+    d.out_m1 = 1;
+    d.out_s0 = N;
+    d.out_s1 = 0;
+    const GemmPlan plan = make_gemm_plan(d);
+    run_gemm(plan, nullptr);
+    B200_CUDA(cudaDeviceSynchronize());
+    B200_CUDA(cudaMemcpy(c, d_c, (size_t)M * N * 2, cudaMemcpyDeviceToHost));
 }
 
 }  // namespace b200

@@ -1,5 +1,6 @@
 // wgmma GEMM with fused epilogue:  out[row(g)][n] = act( sum_k A[g][k] * W[n][k] + bias[n] ), fp16 in/out (or E4M3
-// operands, GemmDesc::fp8), fp32 accumulation in registers.  See gemm.cu.
+// operands, GemmDesc::fp8), fp32 accumulation in registers; or int8 operands with exact s32 accumulation and a per-column
+// dequantisation factor (GemmDesc::q8).  See gemm.cu.
 #pragma once
 
 #include "tc.cuh"
@@ -16,10 +17,25 @@ enum GemmAct : int {
     GEMM_ACT_ROPE = 5,         // output columns are [3][H][64] (q|k|v): rotary embedding on q and k (TxModules.cpp:220-250)
 };
 
+// The int8 precision of the LSTM models (GemmDesc::q8)
+enum GemmQ8 : int {
+    GEMM_Q8_NONE = 0,
+    GEMM_Q8_OPERANDS = 1,  // A and W are int8: exact s32 accumulation, out = act(float(acc) * col_scale[n] + bias[n]) as fp16
+    GEMM_Q8_STORE = 2,     // fp16 operands, GEMM_ACT_TANH: the output is int8 cvt.rni.sat(kInt8ActScale * tanh(v))
+};
+// int8 value of an activation v in [-1, 1] (the last convolution's tanh output and every h_t of an int8 LSTM layer).  The
+// reference's factor is inside closed Koi; 127 is this engine's choice: the symmetric range, so -128 never appears.
+constexpr float kInt8ActScale = 127.0f;
+
 struct GemmDesc {
     // fp8 = 1: A and W are E4M3 bytes (K a multiple of 128, one 128-byte TMA box row per K block), and the SwiGLU epilogue
     // writes E4M3; every other epilogue writes fp16.  Only GEMM_ACT_NONE and GEMM_ACT_SWIGLU have E4M3 forms.
     int fp8 = 0;
+    // q8: GemmQ8.  GEMM_Q8_OPERANDS takes int8 bytes with the E4M3 form's addressing (K a multiple of 128), the plain and
+    // TANH_X5 activations, a column bias and col_scale [N] (fp32 dequantisation factor per output column).
+    // GEMM_Q8_STORE writes int8 where the fp16 form writes fp16: out is int8 and its strides count bytes.
+    int q8 = GEMM_Q8_NONE;
+    const float* col_scale = nullptr;
     // A: logical [batches][rows_per_batch][K] fp16, K contiguous; row/batch strides in elements
     const void* a = nullptr;
     int batches = 1;

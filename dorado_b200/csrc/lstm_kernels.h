@@ -34,13 +34,19 @@ void launch_conv12(const Conv12Params& p, cudaStream_t stream);
 // One LSTM layer's weights on the device.  lstm_size 96 (lstm_layer_kernel): W_ih [4C][C], W_hh and the bias with their
 // gate rows permuted for the fused kernel.  Other sizes: PyTorch gate order (i | f | g | o), W_ih [4C][C padded to a
 // multiple of 64] for the x-projection GEMM.
+// The int8 form (upload_lstm_layer_int8; lstm_size 256 and 384): w_ih8 and w_hh8 [4C][C] int8, quantised together per gate
+// row, inv [4C] the fp32 factor that dequantises a row's s32 accumulator, and the bias; w_ih and w_hh stay null.
 struct LstmLayerWeights {
     __half* w_ih = nullptr;
     __half* w_hh = nullptr;  // [4C][C]
     float* bias = nullptr;   // [4C] b_ih + b_hh (fp32)
+    int8_t* w_ih8 = nullptr;
+    int8_t* w_hh8 = nullptr;
+    float* inv = nullptr;
 };
 // fp32 PyTorch layouts (W_ih and W_hh [4C][C], b_ih and b_hh [4C]) -> the device layout for lstm_size C
 LstmLayerWeights upload_lstm_layer(int C, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh);
+LstmLayerWeights upload_lstm_layer_int8(int C, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh);
 void free_lstm_layer(LstmLayerWeights& w);
 
 struct LstmStackDesc {
@@ -50,7 +56,10 @@ struct LstmStackDesc {
     int stride = 1;              // samples per step, for the chunk lengths of set_chunk_lengths
     int runners = 1;             // batches in flight: sizes the grid recurrence and caps the x-projection GEMM's CTAs
     bool reverse_first = false;  // layer 0 (and every other layer after it) runs reversed in time
-    __half* seq = nullptr;       // [T + 1][Np][C]: the first layer's input, overwritten in place with h by every layer
+    // int8 layers (lstm_size 256 and 384): seq holds int8 cvt.rni.sat.s8(kInt8ActScale * v), the x-projection and the
+    // recurrence run on int8 operands with s32 accumulation (lstm_rec_i8_kernel), gx stays fp16
+    bool int8 = false;
+    void* seq = nullptr;         // [T + 1][Np][C] fp16 (int8 if `int8`): the first layer's input, overwritten in place with h by every layer
     const LstmLayerWeights* layers = nullptr;  // kept by the caller for the stack's lifetime
     int num_layers = 0;
 };
@@ -66,7 +75,8 @@ class Bump;
 LstmStackBuffers carve_lstm_stack(Bump& b, int C, int num_layers, int T, int Np);
 
 // Every layer is lstm_layer_kernel (lstm_size 96), or the x-projection GEMM followed by lstm_rec_kernel (128 - 384) or by
-// one or more cooperative launches of lstm_grid_rec_kernel (768, 1024).  Built once per batch shape; reads
+// one or more cooperative launches of lstm_grid_rec_kernel (768, 1024); int8 layers are the int8 x-projection GEMM followed
+// by lstm_rec_i8_kernel.  Built once per batch shape; reads
 // B200_DEBUG_LSTM_LAYERS, B200_CLUSTER_CHUNKS, B200_GRID_CHUNKS and B200_GRID_GROUPS then.
 class LstmStack {
 public:

@@ -9,6 +9,9 @@
 //                                                                                         256, 384),
 //                                                                                         gx GEMM + lstm_grid_rec_kernel (768, 1024)
 //   LinearCRF              host_linear                       dorado/nn/CRFModules.cpp:49-122   -> gemm.cu
+//   int8 (CUTLASS_TNC_I8)  the same call sites with KOI_I8   ConvStack.cpp:66-74, LSTMStack.cpp:127-211, CRFModules.cpp:103-117
+//                                                                                      -> the int8 forms of gemm.cu +
+//                                                                                         lstm_rec_i8_kernel (256, 384; opt-in)
 // Semantics are those of the CPU modules (ConvStack.cpp:146-163, LSTMStack.cpp:29-41, CRFModules.cpp:24-34).
 //
 // The LSTM layers run through LstmStack (declared in lstm_kernels.h), which owns the layer weights' device layout, the
@@ -18,7 +21,8 @@
 // Activation layouts in HBM (fp16):
 //   signal  [N][T_in]
 //   x2      [N][T_in + 2*pad3 + 8][16]      conv2 output, NTC, zero rows = conv3's padding (+ K padding)
-//   seq     [T_out][N][C]                   time-major LSTM buffer, updated in place by every layer
+//   seq     [T_out][N][C]                   time-major LSTM buffer, updated in place by every layer (int8 in the int8_lstm
+//                                           precision: cvt.rni.sat.s8(kInt8ActScale * v) of conv3's tanh output and every h_t)
 //   scores  [N][T_out][outsize]
 #include "engine.h"
 #include "gemm.h"
@@ -27,6 +31,7 @@
 #include "tc.cuh"
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -680,6 +685,168 @@ __global__ void __launch_bounds__(RecCfg<C, CL, NB>::THREADS, 1) lstm_rec_kernel
 }
 
 // ------------------------------------------------------------------------------------------------
+// The recurrence on int8 operands (lstm_rec_i8_kernel; lstm_size 256 and 384, the int8_lstm precision).
+//
+// The structure of lstm_rec_kernel: one launch per layer, a cluster of CL CTAs per NB chunks, one cluster barrier per step,
+// h double-buffered, per-chunk lengths through the same multiplicative mask.  What differs:
+//   * W_hh rows are int8 (quantised per gate row, quantize_rows_f16) and stay in registers as mma.sync m16n8k32 A fragments:
+//     C / 32 x 4 registers per thread, half of the fp16 kernel's;
+//   * h is int8 in shared memory and in the sequence buffer.  A row of h is C bytes at a stride of C + 16: an ldmatrix
+//     8x8 b16 tile reads 16 bytes of K from each of 8 chunk rows, which is the s8 B fragment, and C + 16 = 16 (mod 128)
+//     puts the eight rows of a phase on distinct banks;
+//   * the s32 accumulator is exact.  The MMA warp converts it and multiplies by inv[row] = 1 / (kInt8ActScale * scale[row])
+//     (fp32), so the gate buffer holds fp32 W_hh h_{t-1} as before, and pre = that + gx;
+//   * h_t is quantised once, cvt.rni.sat.s8(kInt8ActScale * h): the same byte pair goes to every CTA's copy of h and to the
+//     sequence buffer.
+// ------------------------------------------------------------------------------------------------
+struct LstmRecI8Params {
+    int8_t* seq;            // [T][N][C] output h (in place over the layer input, which gx has consumed)
+    const __half* gx;       // [T][N][4C]
+    const int8_t* w_hh;     // [4C][C], PyTorch row order
+    const float* inv;       // [4C] dequantisation factor of a gate row's accumulator
+    int T, N, reverse;
+    const int32_t* lens;    // optional per-chunk length in samples (variable chunk sizes); stride = samples per step
+    int stride;
+};
+
+template <int C, int CL, int NB>
+struct RecI8Cfg {
+    static constexpr int U = C / CL;              // hidden units per CTA
+    static constexpr int MT = 4 * U / 16;         // m16 tiles of gate rows = warps
+    static constexpr int THREADS = 32 * MT;
+    static constexpr int KS = C / 32;             // K steps
+    static constexpr int NT = NB / 8;             // n8 tiles of chunks
+    static constexpr int HS = C + 16;             // row stride of h in bytes: the 8 rows of an ldmatrix phase on distinct banks
+    static constexpr int GS = NB + 4;             // row stride of the gate pre-activations (fp32)
+    static constexpr int PAIRS = U / 2 * NB / THREADS;   // (unit pair, chunk) cells per thread
+    static constexpr bool GX_AHEAD = PAIRS <= 2;  // as RecCfg: gx ahead of the MMAs while it fits the registers
+    static constexpr size_t SMEM = (size_t)2 * NB * HS + (size_t)4 * U * GS * 4;
+    static_assert(C % 32 == 0 && C % CL == 0 && U % 4 == 0 && NT % 2 == 0 && PAIRS >= 1 && (U / 2 * NB) % THREADS == 0, "recurrence shape");
+    static_assert(HS % 128 == 16 && THREADS <= 1024 && CL > 1 && CL <= 8, "h stride / block / cluster size");
+};
+
+template <int C, int CL, int NB>
+__global__ void __launch_bounds__(RecI8Cfg<C, CL, NB>::THREADS, 1) lstm_rec_i8_kernel(const LstmRecI8Params p) {
+    using Cfg = RecI8Cfg<C, CL, NB>;
+    constexpr int U = Cfg::U, KS = Cfg::KS, NT = Cfg::NT, HS = Cfg::HS, GS = Cfg::GS, PAIRS = Cfg::PAIRS;
+    constexpr bool GX_AHEAD = Cfg::GX_AHEAD;
+    extern __shared__ __align__(16) uint8_t smem_raw[];
+    int8_t* h_s = reinterpret_cast<int8_t*>(smem_raw);                          // [2][NB][HS]  this CTA's copy of h
+    float* g_s = reinterpret_cast<float*>(smem_raw + (size_t)2 * NB * HS);      // [4U][GS]
+    __shared__ int len_s[NB];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    cg::cluster_group cluster = cg::this_cluster();
+    const int rank = (int)cluster.block_rank();
+    const int n0 = (int)(blockIdx.x / CL) * NB;
+    if (threadIdx.x < NB) len_s[threadIdx.x] = p.lens ? min(p.T, __ldg(p.lens + n0 + threadIdx.x) / p.stride) : p.T;
+    for (int i = threadIdx.x; i < 2 * NB * HS / 16; i += Cfg::THREADS) reinterpret_cast<uint4*>(h_s)[i] = make_uint4(0, 0, 0, 0);
+
+    // A fragments: local gate row r <-> W_hh row (r / U) * C + rank * U + r % U
+    uint32_t a[KS][4];
+    float inv_lo, inv_hi;
+    {
+        const int r_lo = warp * 16 + (lane >> 2), r_hi = r_lo + 8;
+        const int g_lo = (r_lo / U) * C + rank * U + r_lo % U, g_hi = (r_hi / U) * C + rank * U + r_hi % U;
+        const int8_t* w_lo = p.w_hh + (size_t)g_lo * C;
+        const int8_t* w_hi = p.w_hh + (size_t)g_hi * C;
+        inv_lo = __ldg(p.inv + g_lo);
+        inv_hi = __ldg(p.inv + g_hi);
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+            const int col = ks * 32 + 4 * (lane & 3);
+            a[ks][0] = __ldg(reinterpret_cast<const unsigned int*>(w_lo + col));
+            a[ks][1] = __ldg(reinterpret_cast<const unsigned int*>(w_hi + col));
+            a[ks][2] = __ldg(reinterpret_cast<const unsigned int*>(w_lo + col + 16));
+            a[ks][3] = __ldg(reinterpret_cast<const unsigned int*>(w_hi + col + 16));
+        }
+    }
+    // cells: pair index q = threadIdx.x + j * THREADS -> units (u, u + 1), u = 2 (q % (U / 2)), chunk q / (U / 2)
+    float c_reg[PAIRS][2];
+#pragma unroll
+    for (int j = 0; j < PAIRS; ++j) c_reg[j][0] = c_reg[j][1] = 0.0f;
+    // every CTA of the cluster has zeroed its copy of h before anybody writes h_0 into it
+    cluster.sync();
+
+    int steps = 0;
+    for (int i = 0; i < NB; ++i) steps = max(steps, len_s[i]);
+    const int qm = lane >> 3, qr = lane & 7;   // ldmatrix: matrix qm = (n tile qm / 2, k half qm % 2), row qr
+    for (int s = 0; s < steps; ++s) {
+        const int t = p.reverse ? steps - 1 - s : s;
+        const int cur = s & 1, nxt = cur ^ 1;
+        auto load_gx = [&](int j, __half2* dst) {
+            const int q = threadIdx.x + j * Cfg::THREADS;
+            const int u = 2 * (q % (U / 2)), n = q / (U / 2);
+            const __half* gp = p.gx + ((size_t)t * p.N + n0 + n) * (4 * C) + rank * U + u;
+#pragma unroll
+            for (int g = 0; g < 4; ++g) dst[g] = *reinterpret_cast<const __half2*>(gp + g * C);
+        };
+        __half2 gxv[GX_AHEAD ? PAIRS : 1][4];
+        if constexpr (GX_AHEAD) {
+#pragma unroll
+            for (int j = 0; j < PAIRS; ++j) load_gx(j, gxv[j]);
+        }
+        int32_t acc[NT][4];
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0;
+        const uint32_t hb = tc::smem_u32(h_s + cur * NB * HS);
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+#pragma unroll
+            for (int np = 0; np < NT / 2; ++np) {
+                uint32_t b[4];
+                const int n = (2 * np + (qm >> 1)) * 8 + qr, k = ks * 32 + (qm & 1) * 16;
+                tc::ldmatrix_x4(b, hb + (uint32_t)(n * HS + k));
+                tc::mma_s8_16832(acc[2 * np], a[ks], b[0], b[1]);
+                tc::mma_s8_16832(acc[2 * np + 1], a[ks], b[2], b[3]);
+            }
+        }
+        {
+            const int r_lo = warp * 16 + (lane >> 2);
+#pragma unroll
+            for (int nt = 0; nt < NT; ++nt) {
+                const int col = nt * 8 + 2 * (lane & 3);
+                *reinterpret_cast<float2*>(g_s + r_lo * GS + col) = make_float2((float)acc[nt][0] * inv_lo, (float)acc[nt][1] * inv_lo);
+                *reinterpret_cast<float2*>(g_s + (r_lo + 8) * GS + col) = make_float2((float)acc[nt][2] * inv_hi, (float)acc[nt][3] * inv_hi);
+            }
+        }
+        __syncthreads();
+#pragma unroll
+        for (int j = 0; j < PAIRS; ++j) {
+            const int q = threadIdx.x + j * Cfg::THREADS;
+            const int u = 2 * (q % (U / 2)), n = q / (U / 2);
+            // outside the chunk (variable chunk sizes) the state is held at zero: a multiplicative mask, not a branch
+            const float alive = t < len_s[n] ? 1.0f : 0.0f;
+            __half2 gxl[4];
+            const __half2* gxj = gxl;
+            if constexpr (GX_AHEAD) gxj = gxv[j];
+            else load_gx(j, gxl);
+            int32_t hq[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                float pre[4];
+#pragma unroll
+                for (int g = 0; g < 4; ++g) {
+                    const float2 x = __half22float2(gxj[g]);
+                    pre[g] = g_s[(g * U + u + e) * GS + n] + (e ? x.y : x.x);
+                }
+                const float ig = gate_act(pre[0], 1.0f), fg = gate_act(pre[1], 1.0f);
+                const float gg = gate_act(pre[2], 2.0f), og = gate_act(pre[3], 1.0f);
+                const float cs = (fg * c_reg[j][e] + ig * gg) * alive;
+                c_reg[j][e] = cs;
+                hq[e] = tc::cvt_rni_sat_s8(kInt8ActScale * (og * tanh_f(cs) * alive));
+            }
+            const uint16_t h2 = (uint16_t)((hq[0] & 0xff) | ((hq[1] & 0xff) << 8));
+            *reinterpret_cast<uint16_t*>(p.seq + ((size_t)t * p.N + n0 + n) * C + rank * U + u) = h2;
+            int8_t* h_own = h_s + (nxt * NB + n) * HS + rank * U + u;
+#pragma unroll
+            for (int r = 0; r < CL; ++r) *reinterpret_cast<uint16_t*>(cluster.map_shared_rank(h_own, r)) = h2;
+        }
+        // h_t has landed in every copy, and every thread is done with h_{t-1} and the gate buffer
+        cluster.sync();
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // lstm_size 768 and 1024: recurrence over a group of CTAs that exchange h through L2 (lstm_grid_rec_kernel).
 //
 // W_hh is 4.5 MiB (768) or 8 MiB (1024) of fp16, more than the registers and shared memory of a cluster, so the weights are
@@ -895,6 +1062,39 @@ void launch_lstm_rec(int C, int nb, int ctas, const LstmRecParams& p, cudaStream
     }
 }
 
+template <int C, int NB>
+static void launch_rec_i8_t(const LstmRecI8Params& rp, int ctas, cudaStream_t stream) {
+    constexpr int CL = rec_cluster(C);
+    using Cfg = RecI8Cfg<C, CL, NB>;
+    ensure_dynamic_smem(lstm_rec_i8_kernel<C, CL, NB>, (int)Cfg::SMEM);
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3((unsigned)ctas, 1, 1);
+    cfg.blockDim = dim3(Cfg::THREADS, 1, 1);
+    cfg.dynamicSmemBytes = Cfg::SMEM;
+    cfg.stream = stream;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = CL;
+    at[0].val.clusterDim.y = 1;
+    at[0].val.clusterDim.z = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+    B200_CUDA(cudaLaunchKernelEx(&cfg, lstm_rec_i8_kernel<C, CL, NB>, rp));
+}
+
+// Launches lstm_rec_i8_kernel<C, cluster, nb> over `ctas` CTAs; throws Unsupported for a size without an instantiation
+void launch_lstm_rec_i8(int C, int nb, int ctas, const LstmRecI8Params& p, cudaStream_t stream) {
+    switch (C * 100 + nb) {
+        case 25616: launch_rec_i8_t<256, 16>(p, ctas, stream); break;
+        case 25632: launch_rec_i8_t<256, 32>(p, ctas, stream); break;
+        case 25664: launch_rec_i8_t<256, 64>(p, ctas, stream); break;
+        case 38416: launch_rec_i8_t<384, 16>(p, ctas, stream); break;
+        case 38432: launch_rec_i8_t<384, 32>(p, ctas, stream); break;
+        case 38464: launch_rec_i8_t<384, 64>(p, ctas, stream); break;
+        default: throw Unsupported("no int8 LSTM recurrence instantiation for this lstm_size");
+    }
+}
+
 // Chunks per cluster: 32 for large batches, 16 below.  64 chunks (B200_CLUSTER_CHUNKS=64) spill registers next to the
 // register-resident W_hh of lstm_size 384 and were no faster: hac batch 512, 4 runners, 77.6 vs 77.7 Msamples/s for 64 vs 32
 // (two alternating runs each, NVIDIA H100 80GB HBM3 at 700 W).
@@ -994,10 +1194,81 @@ LstmLayerWeights upload_lstm_layer(int C, const float* w_ih, const float* w_hh, 
     return w;
 }
 
+// utils::quantize_tensor(w, 1) (torch_utils/tensor_utils.cpp:293-300) as torch evaluates it on an fp16 tensor: every
+// operation computes in fp32 and rounds its result to fp16.  128 / absmax, the product w * scale and its rounding to the
+// nearest integer (ties to even) are all fp16 values.  An all-zero row gives the reference 128 / 0 = inf and NaN products;
+// here such a row gets q = 0, and its callers give it a dequantisation factor of 0.
+static float f16_to_float(uint16_t bits) {
+    __half_raw r;
+    r.x = bits;
+    return __half2float(__half(r));
+}
+void quantize_rows_f16(const uint16_t* w16, int rows, int cols, int8_t* q, uint16_t* scale16) {
+    for (int r = 0; r < rows; ++r) {
+        const uint16_t* w = w16 + (size_t)r * cols;
+        float absmax = 0.0f;
+        for (int c = 0; c < cols; ++c) absmax = std::max(absmax, std::fabs(f16_to_float(w[c])));
+        scale16[r] = f16_bits(128.0f / absmax);   // +inf for an all-zero row
+        const float scale = f16_to_float(scale16[r]);
+        for (int c = 0; c < cols; ++c) {
+            if (absmax == 0.0f) {
+                q[(size_t)r * cols + c] = 0;
+                continue;
+            }
+            const float prod = f16_to_float(f16_bits(f16_to_float(w[c]) * scale));
+            q[(size_t)r * cols + c] = (int8_t)std::min(127.0f, std::max(-127.0f, std::nearbyintf(prod)));
+        }
+    }
+}
+// Factor that turns an s32 accumulator of int8 activations (kInt8ActScale * v) and a row's int8 weights back into W v
+float int8_row_inv(uint16_t scale16) {
+    const float s = f16_to_float(scale16);
+    return std::isinf(s) ? 0.0f : 1.0f / (kInt8ActScale * s);
+}
+
+template <typename T>
+static T* upload_raw(const std::vector<T>& v) {
+    T* d = nullptr;
+    B200_CUDA(cudaMalloc(&d, v.size() * sizeof(T)));
+    B200_CUDA(cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+    return d;
+}
+
+// The int8 form (lstm_size 256 and 384): fp16(W_ih) | fp16(W_hh) quantised as one [4C][2C] matrix, one scale per gate row
+// of both (LSTMStack.cpp:150-166)
+LstmLayerWeights upload_lstm_layer_int8(int C, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh) {
+    const int R = 4 * C;
+    std::vector<uint16_t> both((size_t)R * 2 * C), scale(R);
+    for (int r = 0; r < R; ++r) {
+        for (int c = 0; c < C; ++c) {
+            both[(size_t)r * 2 * C + c] = f16_bits(w_ih[(size_t)r * C + c]);
+            both[(size_t)r * 2 * C + C + c] = f16_bits(w_hh[(size_t)r * C + c]);
+        }
+    }
+    std::vector<int8_t> q((size_t)R * 2 * C), qi((size_t)R * C), qh((size_t)R * C);
+    quantize_rows_f16(both.data(), R, 2 * C, q.data(), scale.data());
+    std::vector<float> inv(R), b(R);
+    for (int r = 0; r < R; ++r) {
+        std::memcpy(&qi[(size_t)r * C], &q[(size_t)r * 2 * C], C);
+        std::memcpy(&qh[(size_t)r * C], &q[(size_t)r * 2 * C + C], C);
+        inv[r] = int8_row_inv(scale[r]);
+        b[r] = b_ih[r] + b_hh[r];
+    }
+    LstmLayerWeights w;
+    w.w_ih8 = upload_raw(qi);
+    w.w_hh8 = upload_raw(qh);
+    w.inv = upload_f32(inv);
+    w.bias = upload_f32(b);
+    return w;
+}
+
 void free_lstm_layer(LstmLayerWeights& w) {
     cudaFree(w.w_ih);
     cudaFree(w.w_hh);
     cudaFree(w.bias);
+    cudaFree(w.w_ih8);
+    cudaFree(w.w_hh8);
+    cudaFree(w.inv);
     w = LstmLayerWeights{};
 }
 
@@ -1015,6 +1286,7 @@ LstmStackBuffers carve_lstm_stack(Bump& b, int C, int num_layers, int T, int Np)
 
 LstmStack::LstmStack(const LstmStackDesc& d, const LstmStackBuffers& ws) : m_d(d), m_ws(ws) {
     const int C = d.C, Np = d.Np;
+    if (d.int8 && C != 256 && C != 384) throw Unsupported("the int8 LSTM layers exist for lstm_size 256 and 384 only");
     if (const char* dbg = std::getenv("B200_DEBUG_LSTM_LAYERS")) m_debug_layers = std::atoi(dbg);
     if (C == FL_C) {  // one lstm_layer_kernel per layer
         m_nb = FL_NB;
@@ -1061,6 +1333,12 @@ LstmStack::LstmStack(const LstmStackDesc& d, const LstmStackBuffers& ws) : m_d(d
         g.w = w.w_ih;
         g.N = 4 * C;
         g.K = (C + 63) / 64 * 64;
+        if (d.int8) {   // rows of int8, K = C = whole 128-byte blocks
+            g.q8 = GEMM_Q8_OPERANDS;
+            g.w = w.w_ih8;
+            g.col_scale = w.inv;
+            g.K = C;
+        }
         g.bias = w.bias;
         g.act = GEMM_ACT_NONE;
         g.out = m_ws.gx;
@@ -1094,17 +1372,26 @@ bool LstmStack::run(cudaStream_t stream, ProfileSink* prof) {
         const int reverse = (l % 2 == 0) == m_d.reverse_first ? 1 : 0;
         if (m_kind == Kind::Layer) {
             lstm_layer_kernel<<<m_groups, FL_THREADS, 0, stream>>>(
-                    LstmLayerParams{m_d.seq, w.w_ih, w.w_hh, w.bias, m_d.T, Np, reverse});
+                    LstmLayerParams{static_cast<__half*>(m_d.seq), w.w_ih, w.w_hh, w.bias, m_d.T, Np, reverse});
             mark("lstm_layer");
             continue;
         }
         run_gemm(m_gx_gemm[l], stream);
+        if (m_d.int8) {
+            mark("lstm_gx_gemm_i8");
+            launch_lstm_rec_i8(C, m_nb, m_groups * m_group_ctas,
+                               LstmRecI8Params{static_cast<int8_t*>(m_d.seq), m_ws.gx, w.w_hh8, w.inv, m_d.T, Np, reverse, m_lens,
+                                               m_d.stride},
+                               stream);
+            mark("lstm_rec_i8");
+            continue;
+        }
         mark("lstm_gx_gemm");
         // launch i covers groups i * m_groups .. of m_nb chunks, with counters of its own (the last may hold fewer groups)
         for (int i = 0; i < m_launches; ++i) {
             const int ctas = std::min(m_groups, Np / m_nb - i * m_groups) * m_group_ctas;
             unsigned int* counters = m_ws.counters ? m_ws.counters + (size_t)l * (Np / 32) + (size_t)i * m_groups : nullptr;
-            const LstmRecParams p{m_d.seq, m_ws.gx, w.w_hh, m_d.T, Np, reverse, m_lens, m_d.stride, i * m_groups * m_nb,
+            const LstmRecParams p{static_cast<__half*>(m_d.seq), m_ws.gx, w.w_hh, m_d.T, Np, reverse, m_lens, m_d.stride, i * m_groups * m_nb,
                                   counters, m_ws.error};
             if (m_kind == Kind::Rec) {
                 launch_lstm_rec(C, m_nb, ctas, p, stream);
@@ -1132,7 +1419,8 @@ std::string LstmStack::info() const {
     const std::string ctas = std::to_string(m_groups * m_group_ctas);
     switch (m_kind) {
         case Kind::Layer: return "lstm_layer.ctas=" + ctas;
-        case Kind::Rec: return "lstm_rec.ctas=" + ctas + ";lstm_rec.chunks_per_cluster=" + std::to_string(m_nb);
+        case Kind::Rec:
+            return "lstm_rec.ctas=" + ctas + ";lstm_rec.chunks_per_cluster=" + std::to_string(m_nb) + (m_d.int8 ? ";lstm.int8=1" : "");
         default:
             return "lstm_grid.ctas=" + ctas + ";lstm_grid.groups=" + std::to_string(m_groups) + ";lstm_grid.chunks_per_group=" +
                    std::to_string(m_nb) + ";lstm_grid.launches_per_layer=" + std::to_string(m_launches);
@@ -1150,7 +1438,7 @@ class LstmPlan final : public ForwardPlan {
 public:
     void run(cudaStream_t stream, ProfileSink* prof) override;
     int launches() const override { return 1 + 1 + lstm->launches() + num_linear; }
-    std::string info() const override { return lstm->info(); }
+    std::string info() const override { return lstm->info(); }   // "lstm.int8=1" among them in the int8_lstm precision
     void set_chunk_lengths(const int32_t* d_lens) override {
         if (!variable) return;  // the mode exists for the models that run variable chunk sizes only
         conv12.lens = d_lens;
@@ -1191,11 +1479,16 @@ public:
     float* bl1 = nullptr;
     __half* wl2 = nullptr;  // decomposition: [outsize][out_features_p]
     int Cp = 0, out1 = 0, out1p = 0;
+    // desc.lstm_precision == B200_LSTM_INT8: int8 sequence buffer, int8 LSTM layers (layers[].w_ih8 ...), and the first
+    // linear on int8 operands: wl1_8 [out1][C] quantised per output row, wl1_inv [out1] (wl1 unused)
+    bool int8 = false;
+    int8_t* wl1_8 = nullptr;
+    float* wl1_inv = nullptr;
 
 private:
     struct Buffers {
         __half* x2;    // conv2 output [N][t_pad][16]: first, the tests read it at offset 0
-        __half* seq;   // [T_out + 1][Np][C]: second, the tests read it right behind x2
+        void* seq;     // [T_out + 1][Np][C] fp16 (int8 in the int8_lstm precision): second, the tests read it right behind x2
         __half* mid;   // decomposition only: [T_out][Np][out_features]
         int* tile_counter;  // conv12_tc_kernel
         LstmStackBuffers lstm;
@@ -1225,6 +1518,17 @@ LstmModel::LstmModel(const b200_model_desc& d, const b200_tensor* tensors, int n
     }
 
     if (d.lstm_layers < 1 || d.lstm_layers > 8) throw std::invalid_argument("bad lstm_layers");
+    int8 = d.lstm_precision == B200_LSTM_INT8;
+    if (int8) {
+        // The reference's CUTLASS_TNC_I8 conditions (ConvStack.cpp:66-74) cut down to the widths lstm_rec_i8_kernel is built for
+        if (C != 256 && C != 384) {
+            throw Unsupported("int8_lstm precision: lstm_size " + std::to_string(C) + " is not supported (256 and 384 are)");
+        }
+        if (c3.activation != B200_ACT_TANH) {
+            throw Unsupported("int8_lstm precision needs a tanh last convolution: the int8 activations assume values in [-1, 1]");
+        }
+        if (d.lstm_inner_dim > 0) throw Unsupported("int8_lstm precision: FLSTM models (lstm_inner_dim > 0) are not supported");
+    }
 
     conv_w = upload_conv12_weights(find_tensor(tensors, n, "0.conv.weight.tensor"), find_tensor(tensors, n, "0.conv.bias.tensor"),
                                    find_tensor(tensors, n, "1.conv.weight.tensor"), find_tensor(tensors, n, "1.conv.bias.tensor"),
@@ -1283,7 +1587,7 @@ LstmModel::LstmModel(const b200_model_desc& d, const b200_tensor* tensors, int n
             bih = find_tensor(tensors, n, pfx + "bias_ih_l0.tensor").data;
             bhh = find_tensor(tensors, n, pfx + "bias_hh_l0.tensor").data;
         }
-        layers.push_back(upload_lstm_layer(C, wih, whh, bih, bhh));
+        layers.push_back(int8 ? upload_lstm_layer_int8(C, wih, whh, bih, bhh) : upload_lstm_layer(C, wih, whh, bih, bhh));
     }
     // linear(s)
     {
@@ -1293,7 +1597,18 @@ LstmModel::LstmModel(const b200_model_desc& d, const b200_tensor* tensors, int n
         Cp = (C + 63) / 64 * 64;
         std::vector<float> w((size_t)out1 * Cp, 0.0f);
         for (int o = 0; o < out1; ++o) std::memcpy(&w[(size_t)o * Cp], &tw.data[(size_t)o * C], sizeof(float) * C);
-        wl1 = upload_f16(w);
+        if (int8) {   // quantised per output row, as CRFModules.cpp:107-109 (C is a multiple of 128: no K padding)
+            std::vector<uint16_t> w16((size_t)out1 * C), scale(out1);
+            for (size_t i = 0; i < w16.size(); ++i) w16[i] = f16_bits(tw.data[i]);
+            std::vector<int8_t> q(w16.size());
+            quantize_rows_f16(w16.data(), out1, C, q.data(), scale.data());
+            std::vector<float> inv(out1);
+            for (int o = 0; o < out1; ++o) inv[o] = int8_row_inv(scale[o]);
+            wl1_8 = upload_raw(q);
+            wl1_inv = upload_f32(inv);
+        } else {
+            wl1 = upload_f16(w);
+        }
         if (d.linear_bias) {
             const auto& tb = find_tensor(tensors, n, std::to_string(layer) + ".linear.bias.tensor");
             bl1 = upload_f32(std::vector<float>(tb.data, tb.data + out1));
@@ -1312,6 +1627,8 @@ LstmModel::~LstmModel() {
     cudaFree(b3);
     for (auto& l : layers) free_lstm_layer(l);
     cudaFree(wl1);
+    cudaFree(wl1_8);
+    cudaFree(wl1_inv);
     cudaFree(bl1);
     cudaFree(wl2);
 }
@@ -1327,7 +1644,7 @@ LstmModel::Buffers LstmModel::carve(Bump& b, int N, int T_in) const {
     }
     Buffers w;
     w.x2 = b.take<__half>((size_t)N * t_pad(T_in) * 16 * 2);
-    w.seq = b.take<__half>((size_t)(T_out + 1) * Np * C * 2);
+    w.seq = b.take((size_t)(T_out + 1) * Np * C * (int8 ? 1 : 2));
     w.mid = desc.out_features > 0 ? b.take<__half>((size_t)T_out * Np * desc.out_features * 2) : nullptr;
     w.tile_counter = b.take<int>(sizeof(int));
     w.lstm = carve_lstm_stack(b, C, desc.lstm_layers, T_out, Np);
@@ -1378,6 +1695,7 @@ std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half*
         g.K = K3p;
         g.bias = b3;
         g.act = desc.convs[2].activation;
+        g.q8 = int8 ? GEMM_Q8_STORE : GEMM_Q8_NONE;
         g.out = seq;
         g.out_m1 = T_out;        // g = n * T_out + t
         g.out_s0 = C;            // n
@@ -1392,6 +1710,7 @@ std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half*
     lstm.stride = desc.stride;
     lstm.runners = num_runners_hint;
     lstm.reverse_first = true;  // CRFModel.cpp:40, LSTMStack.cpp:31-41
+    lstm.int8 = int8;
     lstm.seq = seq;
     lstm.layers = layers.data();
     lstm.num_layers = desc.lstm_layers;
@@ -1409,6 +1728,12 @@ std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half*
         g.K = Cp;
         g.a_inner = C;
         g.bias = bl1;
+        if (int8) {
+            g.q8 = GEMM_Q8_OPERANDS;
+            g.w = wl1_8;
+            g.col_scale = wl1_inv;
+            g.K = C;
+        }
         if (desc.out_features > 0) {
             g.act = GEMM_ACT_NONE;
             g.out = mid;

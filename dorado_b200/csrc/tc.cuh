@@ -183,6 +183,19 @@ __device__ __forceinline__ void wgmma_m64n32k32_e4m3(float* d, uint64_t adesc, u
             : "l"(adesc), "l"(bdesc), "r"((uint32_t)accumulate)
             : "memory");
 }
+// The same tile for int8 operands: D[64 x 32] (+)= A[64 x 32] B[32 x 32]^T, K-major, exact s32 accumulation.  Addressing
+// and the accumulator fragment layout are those of the E4M3 form; the integer form takes no operand scale or transpose.
+__device__ __forceinline__ void wgmma_m64n32k32_s8(int32_t* d, uint64_t adesc, uint64_t bdesc, bool accumulate) {
+    asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %18, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 "
+            "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p;\n\t}"
+            : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]),
+              "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+            : "l"(adesc), "l"(bdesc), "r"((uint32_t)accumulate)
+            : "memory");
+}
 // Two fp32 values to E4M3 (round to nearest even; beyond +-448 saturates to +-448, NaN stays NaN): lo in the low byte.
 __device__ __forceinline__ uint16_t cvt_e4m3x2(float lo, float hi) {
     uint16_t r;
@@ -198,6 +211,21 @@ __device__ __forceinline__ void mma_f16_16816(float* c, const uint32_t* a, uint3
     asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
                  : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+// m16n8k32 on int8, exact s32 accumulation: a[4] = A rows (l / 4, + 8) x 4 bytes of k at 4 (l % 4) (+ 16); b[2] = B 4 bytes of
+// k at 4 (l % 4) (+ 16) x column l / 4; c[4] as m16n8k16.  An ldmatrix 8x8 b16 tile whose rows are 16 bytes of k gives the
+// b fragment: thread l gets bytes 4 (l % 4) .. + 3 of row l / 4.
+__device__ __forceinline__ void mma_s8_16832(int32_t* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+// The int8 activation quantiser: round(v) to nearest even, saturated to [-128, 127] (callers pass kInt8ActScale * v with
+// |v| <= 1, so -128 is never produced)
+__device__ __forceinline__ int32_t cvt_rni_sat_s8(float v) {
+    int32_t r;
+    asm("cvt.rni.sat.s8.f32 %0, %1;" : "=r"(r) : "f"(v));
+    return r;
 }
 __device__ __forceinline__ void ldmatrix_x4(uint32_t* r, uint32_t smem_addr) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
@@ -233,7 +261,7 @@ __device__ __forceinline__ uint32_t sw128_offset(int row, int chunk16) {
 
 // ---------------------------------------------------------------- host: tensor maps
 // cuTensorMapEncodeTiled through the runtime's driver entry point (no link dependency on libcuda).  Elements are fp16, or
-// bytes (E4M3) when elem_bytes == 1; a box row of 128 bytes gets the 128-byte swizzle.
+// bytes (E4M3 or int8) when elem_bytes == 1; a box row of 128 bytes gets the 128-byte swizzle.
 CUtensorMap make_tmap_2d(const void* base, uint64_t inner, uint64_t outer, uint64_t outer_stride_bytes, uint32_t box_inner,
                          uint32_t box_outer, uint32_t elem_bytes = 2);
 CUtensorMap make_tmap_3d(const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t s1_bytes, uint64_t s2_bytes,

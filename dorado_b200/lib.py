@@ -42,12 +42,12 @@ class ModelDesc(C.Structure):
         ("attn_window_upper", C.c_int32), ("attn_window_lower", C.c_int32),
         ("upsample_scale", C.c_int32), ("max_seq_len", C.c_int32),
         ("deepnorm_alpha", C.c_float), ("theta", C.c_float), ("tx_crf_scale", C.c_float),
-        ("lstm_inner_dim", C.c_int32), ("tx_precision", C.c_int32),
+        ("lstm_inner_dim", C.c_int32), ("tx_precision", C.c_int32), ("lstm_precision", C.c_int32),
     ]
 
 
-# b200_model_desc.tx_precision
-TX_PRECISIONS = {"fp16": 0, "fp8_ffn": 1}
+# precision name -> (b200_model_desc.tx_precision, b200_model_desc.lstm_precision)
+PRECISIONS = {"fp16": (0, 0), "fp8_ffn": (1, 0), "int8_lstm": (0, 1)}
 
 
 class Tensor(C.Structure):
@@ -90,17 +90,17 @@ class Stats(C.Structure):
 
 
 EXPORTS = [
-    "b200_last_error", "b200_version", "b200_device_count", "b200_default_decoder_options", "b200_engine_create",
+    "b200_last_error", "b200_version", "b200_device_count", "b200_default_decoder_options", "b200_engine_create", "b200_engine_create_sized",
     "b200_engine_destroy", "b200_engine_get_stats", "b200_runner_create", "b200_runner_destroy",
     "b200_runner_set_decoder_options", "b200_runner_batch_size", "b200_runner_chunk_size", "b200_runner_out_len",
     "b200_runner_accept_chunk_f16", "b200_runner_accept_chunk_f32", "b200_runner_input", "b200_runner_call_chunks",
     "b200_runner_upload", "b200_runner_step_device", "b200_runners_step_device", "b200_runner_forward_scores", "b200_runner_profile", "b200_runner_plan_info", "b200_runner_debug_read_workspace", "b200_decode_scores",
-    "b200_test_gemm", "b200_test_gemm_fp8", "b200_test_to_e4m3", "b200_test_remove_bits", "b200_test_attention", "b200_generate_chunks", "b200_stitch_chunks", "b200_runner_accept_raw_chunk",
+    "b200_test_gemm", "b200_test_gemm_fp8", "b200_test_gemm_s8", "b200_test_quantize_rows", "b200_test_to_e4m3", "b200_test_remove_bits", "b200_test_attention", "b200_generate_chunks", "b200_stitch_chunks", "b200_runner_accept_raw_chunk",
     "b200_runner_debug_read_input", "b200_engine_runner_bytes", "b200_engine_benchmark_batch_sizes",
     "b200_select_batch_size", "b200_generate_variable_chunks", "b200_engine_terminate", "b200_engine_restart",
     "b200_engine_set_low_latency", "b200_engine_is_low_latency", "b200_engine_batch_timeouts_ms",
     "b200_engine_set_num_runners", "b200_engine_num_runners",
-    "b200_pool_create", "b200_pool_destroy", "b200_pool_num_runners", "b200_pool_runner", "b200_pool_out_len",
+    "b200_pool_create", "b200_pool_create_sized", "b200_pool_destroy", "b200_pool_num_runners", "b200_pool_runner", "b200_pool_out_len",
     "b200_pool_runner_info", "b200_pool_call_chunks", "b200_runner_variable_chunk_sizes",
     "b200_runner_accept_chunk_var_f16", "b200_chunk_benchmarks_lookup", "b200_engine_gpu_name",
     "b200_modbase_engine_create", "b200_modbase_engine_destroy", "b200_modbase_runner_create", "b200_modbase_runner_destroy",
@@ -132,6 +132,8 @@ def load_library() -> C.CDLL:
     lib.b200_default_decoder_options.argtypes = [C.POINTER(DecoderOptions)]
     lib.b200_pool_create.argtypes = [C.POINTER(ModelDesc), C.POINTER(Tensor), i32, C.POINTER(i32), i32, i32, i32, i32,
                                      C.POINTER(vp)]
+    lib.b200_pool_create_sized.argtypes = [C.POINTER(ModelDesc), C.c_size_t, C.POINTER(Tensor), i32, C.POINTER(i32), i32, i32, i32,
+                                           i32, C.POINTER(vp)]
     lib.b200_pool_destroy.argtypes = [vp]
     lib.b200_pool_num_runners.argtypes = [vp]
     lib.b200_pool_out_len.argtypes = [vp]
@@ -154,6 +156,7 @@ def load_library() -> C.CDLL:
     lib.b200_engine_is_low_latency.restype = i32
     lib.b200_engine_batch_timeouts_ms.argtypes = [vp, C.POINTER(i32), C.POINTER(i32)]
     lib.b200_engine_create.argtypes = [C.POINTER(ModelDesc), C.POINTER(Tensor), i32, i32, C.POINTER(vp)]
+    lib.b200_engine_create_sized.argtypes = [C.POINTER(ModelDesc), C.c_size_t, C.POINTER(Tensor), i32, i32, C.POINTER(vp)]
     lib.b200_engine_destroy.argtypes = [vp]
     lib.b200_engine_get_stats.argtypes = [vp, C.POINTER(Stats)]
     lib.b200_runner_create.argtypes = [vp, i32, i32, C.POINTER(vp)]
@@ -178,6 +181,8 @@ def load_library() -> C.CDLL:
     lib.b200_test_gemm.argtypes = [i32, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.b200_test_attention.argtypes = [i32, vp, i32, i32, i32, i32, i32, vp]
     lib.b200_test_gemm_fp8.argtypes = [i32, vp, vp, i32, i32, i32, i32, vp, f32, vp]
+    lib.b200_test_gemm_s8.argtypes = [i32, vp, vp, vp, vp, i32, i32, i32, i32, vp]
+    lib.b200_test_quantize_rows.argtypes = [vp, i32, i32, vp, vp]
     lib.b200_test_to_e4m3.argtypes = [vp, C.c_int64, vp]
     lib.b200_test_remove_bits.argtypes = [vp, C.c_int64, i32, vp]
     u64 = C.c_uint64
@@ -210,11 +215,12 @@ def check(status: int) -> None:
 
 
 def model_desc_from_config(cfg: BasecallModelConfig, precision: str = "fp16") -> ModelDesc:
-    """precision: the transformer precision, "fp16" (default) or "fp8_ffn" (E4M3 feed-forward GEMMs, b200call.h)."""
-    if precision not in TX_PRECISIONS:
-        raise ValueError(f"precision must be one of {sorted(TX_PRECISIONS)}, got {precision!r}")
+    """precision: "fp16" (default), "fp8_ffn" (transformer models: E4M3 feed-forward GEMMs) or "int8_lstm" (LSTM models
+    of lstm_size 256 / 384: int8 LSTM layers and CRF linear); see tx_precision and lstm_precision in b200call.h."""
+    if precision not in PRECISIONS:
+        raise ValueError(f"precision must be one of {sorted(PRECISIONS)}, got {precision!r}")
     d = ModelDesc()
-    d.tx_precision = TX_PRECISIONS[precision]
+    d.tx_precision, d.lstm_precision = PRECISIONS[precision]
     d.model_type = 1 if cfg.is_tx_model else 0
     d.num_convs = len(cfg.convs)
     for i, c in enumerate(cfg.convs):
@@ -304,6 +310,35 @@ def test_gemm_fp8(a: np.ndarray, b: np.ndarray, activation: int = -1, residual: 
         res_p = residual.ctypes.data
     check(lib.b200_test_gemm_fp8(device, a.ctypes.data, b.ctypes.data, M, N, K, activation, res_p, alpha, c.ctypes.data))
     return c
+
+
+def test_gemm_s8(a: np.ndarray, b: np.ndarray, col_scale: np.ndarray, bias: np.ndarray | None = None, activation: int = -1,
+                 device: int = 0):
+    """The int8 GEMM on host data: a [M, K], b [N, K] int8 -> fp16 [M, N] of act(float(a b^T) * col_scale + bias)."""
+    lib = load_library()
+    a = np.ascontiguousarray(a, np.int8)
+    b = np.ascontiguousarray(b, np.int8)
+    M, K = a.shape
+    N = b.shape[0]
+    col_scale = np.ascontiguousarray(col_scale, np.float32)
+    assert col_scale.shape == (N,)
+    bias_p = None
+    if bias is not None:
+        bias = np.ascontiguousarray(bias, np.float32)
+        bias_p = bias.ctypes.data
+    c = np.empty((M, N), np.float16)
+    check(lib.b200_test_gemm_s8(device, a.ctypes.data, b.ctypes.data, col_scale.ctypes.data, bias_p, M, N, K, activation,
+                                c.ctypes.data))
+    return c
+
+
+def quantize_rows(w: np.ndarray):
+    """The engine's host quantisation of fp16 values [rows, cols] (no device needed): (int8 [rows, cols], fp16 scale [rows])."""
+    h = np.ascontiguousarray(w, np.float16)
+    q = np.empty(h.shape, np.int8)
+    scale = np.empty(h.shape[0], np.float16)
+    check(load_library().b200_test_quantize_rows(h.ctypes.data, h.shape[0], h.shape[1], q.ctypes.data, scale.ctypes.data))
+    return q, scale
 
 
 def to_e4m3(x: np.ndarray) -> np.ndarray:

@@ -37,7 +37,8 @@ class B200Caller:
 
     def __init__(self, cfg: BasecallModelConfig, weights: dict, device: int = 0, low_latency: bool = False,
                  num_runners: int = 2, precision: str = "fp16"):
-        """precision: transformer precision, "fp16" or "fp8_ffn" (fc1 / fc2 on E4M3 operands; include/b200call.h)."""
+        """precision: "fp16", "fp8_ffn" (transformer models: fc1 / fc2 on E4M3 operands) or "int8_lstm" (LSTM models of
+        lstm_size 256 / 384: int8 LSTM layers and CRF linear); include/b200call.h."""
         self.cfg = cfg
         self.device = device
         self.precision = precision
@@ -54,7 +55,7 @@ class B200Caller:
             for k, dim in enumerate(w.shape):
                 arr[i].dims[k] = dim
         self.handle = C.c_void_p()
-        L.check(lib.b200_engine_create(C.byref(desc), arr, len(weights), device, C.byref(self.handle)))
+        L.check(lib.b200_engine_create_sized(C.byref(desc), C.sizeof(desc), arr, len(weights), device, C.byref(self.handle)))
         self._keep = None  # the engine copied everything to the device
         L.check(lib.b200_engine_set_low_latency(self.handle, int(low_latency)))
         # api::create_basecall_runners' num_runners (api/runner_creation.cpp:46-130): shapes launch plans only
@@ -138,8 +139,8 @@ class B200Pool:
         self.chunk_size = cfg.normalise_chunk_size(chunk_size)
         self.batch_size = batch_size
         self.handle = C.c_void_p()
-        L.check(lib.b200_pool_create(C.byref(desc), arr, len(weights), devs, len(devices), runners_per_device, batch_size,
-                                     self.chunk_size, C.byref(self.handle)))
+        L.check(lib.b200_pool_create_sized(C.byref(desc), C.sizeof(desc), arr, len(weights), devs, len(devices),
+                                           runners_per_device, batch_size, self.chunk_size, C.byref(self.handle)))
         del keep
         self.t_out = lib.b200_pool_out_len(self.handle)
 

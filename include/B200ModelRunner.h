@@ -23,6 +23,7 @@
 #include <ATen/ATen.h>
 
 #include <atomic>
+#include <cstdlib>
 #include <memory>
 #include <stdexcept>
 #include <string>
@@ -74,6 +75,15 @@ public:
             // path is the one held to the oracle.  koi_use_i8 and other remove_bits values have no counterpart.
             if (utils::get_dev_opt<bool>("koi_use_f8", false)) {
                 d.tx_precision = B200_TX_FP8_FFN;
+            }
+        }
+        // The reference's own override (ConvStack.cpp:77-87): DORADO_LSTM_MODE=CUTLASS_TNC_I8 selects the int8 LSTM layers
+        // (b200call.h, lstm_precision).  The reference runs hac that way by default; here fp16 is the default and the mode is
+        // taken only when asked for, on the shapes the engine has it for (others fail engine creation).
+        if (!model_config.is_tx_model()) {
+            const char* lstm_mode = std::getenv("DORADO_LSTM_MODE");
+            if (lstm_mode != nullptr && std::string(lstm_mode) == "CUTLASS_TNC_I8") {
+                d.lstm_precision = B200_LSTM_INT8;
             }
         }
         // Weights: the reference's own loader (crf_utils.cpp:26-150) gives the tensors in file-list order; the

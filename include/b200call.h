@@ -39,6 +39,8 @@ enum { B200_ACT_SWISH = 0, B200_ACT_SWISH_CLAMP = 1, B200_ACT_TANH = 2 };
 enum { B200_MODEL_LSTM = 0, B200_MODEL_TX = 1 };
 /* transformer precision (b200_model_desc.tx_precision) */
 enum { B200_TX_FP16 = 0, B200_TX_FP8_FFN = 1 };
+/* LSTM precision (b200_model_desc.lstm_precision) */
+enum { B200_LSTM_FP16 = 0, B200_LSTM_INT8 = 1 };
 
 /* config::ConvParams (dorado/config/include/config/common.h) */
 typedef struct b200_conv_desc {
@@ -82,6 +84,17 @@ typedef struct b200_model_desc {
      * in whole 128-byte E4M3 blocks; the engine does not pad it): others return B200_ERR_UNSUPPORTED.  On an LSTM model,
      * or any other value, b200_engine_create returns B200_ERR_INVALID.  b200_runner_plan_info reports "tx.fp8_ffn=1". */
     int32_t tx_precision;
+    /* LSTM precision.  B200_LSTM_FP16 (0, what a zero-initialised descriptor gets): fp16 operands, fp32 accumulation.
+     * B200_LSTM_INT8 (1): the reference's CUTLASS_TNC_I8 layout (dorado/nn/ConvStack.cpp:66-74, LSTMStack.cpp:127-211,
+     * CRFModules.cpp:103-117), its default for hac.  Per LSTM layer fp16(W_ih) | fp16(W_hh) are quantised to int8 as one
+     * [4C, 2C] matrix with one fp16 scale per gate row (utils::quantize_tensor, evaluated in fp16 as the reference does); the
+     * first CRF linear's weight likewise per output row.  The last convolution's tanh output and every h_t are stored as int8
+     * round(127 v); the x-projection, the recurrence and that linear accumulate exactly in s32 and dequantise per row in fp32;
+     * gx, the cell state and the scores keep their fp16 / fp32 types.  A second linear (out_features) stays fp16.  Shapes:
+     * plain LSTM models with lstm_size 256 or 384 and a tanh last convolution; lstm_size 96 / 128 / 192 / 768 / 1024, another
+     * last activation and FLSTM models return B200_ERR_UNSUPPORTED.  On a transformer model, or any other value,
+     * b200_engine_create returns B200_ERR_INVALID.  b200_runner_plan_info reports "lstm.int8=1". */
+    int32_t lstm_precision;
 } b200_model_desc;
 
 /* Host fp32 tensors, named and ordered as the reference's *.tensor files
@@ -138,11 +151,26 @@ B200_API int b200_device_count(void);
 B200_API void b200_default_decoder_options(b200_decoder_options* opts);
 
 /* CudaCaller::CudaCaller (CudaCaller.cpp:149-202): upload + re-lay-out weights on `device`. */
+/* b200_model_desc grows by trailing fields, so the library has to know how much of it the caller's header declares:
+ * b200_engine_create_sized reads desc_size bytes and takes every field beyond them as zero (a descriptor longer than the
+ * library's own must be zero there, or B200_ERR_UNSUPPORTED).  b200_engine_create(desc, ...) in source compiled against
+ * this header is b200_engine_create_sized(desc, sizeof(b200_model_desc), ...) (the macro below).  The exported symbol
+ * b200_engine_create serves binaries built against earlier headers, which pass a shorter descriptor: it reads the fields
+ * up to and including tx_precision, so such a binary keeps running in fp16 without being rebuilt.  The same holds for
+ * b200_pool_create. */
+B200_API int b200_engine_create_sized(const b200_model_desc* desc,
+                                      size_t desc_size,
+                                      const b200_tensor* tensors,
+                                      int32_t num_tensors,
+                                      int32_t device,
+                                      b200_engine** out);
 B200_API int b200_engine_create(const b200_model_desc* desc,
                                 const b200_tensor* tensors,
                                 int32_t num_tensors,
                                 int32_t device,
                                 b200_engine** out);
+#define b200_engine_create(desc, tensors, num_tensors, device, out) \
+    b200_engine_create_sized((desc), sizeof(b200_model_desc), (tensors), (num_tensors), (device), (out))
 B200_API int b200_engine_destroy(b200_engine* engine);
 B200_API int b200_engine_get_stats(const b200_engine* engine, b200_stats* out);
 
@@ -335,6 +363,17 @@ B200_API int b200_select_batch_size(const int32_t* batch_sizes,
  * (dynamic load balance; no collective, no inter-GPU traffic), results land in the caller's arrays with row pitch
  * b200_pool_out_len().  Blocking; returns the wall time in *seconds. */
 typedef struct b200_pool b200_pool;
+B200_API int b200_pool_create_sized(const b200_model_desc* desc,
+                                    size_t desc_size,
+                                    const b200_tensor* tensors,
+                                    int32_t num_tensors,
+                                    const int32_t* devices,
+                                    int32_t num_devices,
+                                    int32_t runners_per_device,
+                                    int32_t batch_size,
+                                    int32_t chunk_size,
+                                    b200_pool** out);
+/* As b200_engine_create: the symbol for binaries built against earlier headers, and the macro for this one. */
 B200_API int b200_pool_create(const b200_model_desc* desc,
                               const b200_tensor* tensors,
                               int32_t num_tensors,
@@ -344,6 +383,9 @@ B200_API int b200_pool_create(const b200_model_desc* desc,
                               int32_t batch_size,
                               int32_t chunk_size,
                               b200_pool** out);
+#define b200_pool_create(desc, tensors, num_tensors, devices, num_devices, runners_per_device, batch_size, chunk_size, out) \
+    b200_pool_create_sized((desc), sizeof(b200_model_desc), (tensors), (num_tensors), (devices), (num_devices),          \
+                           (runners_per_device), (batch_size), (chunk_size), (out))
 B200_API int b200_pool_destroy(b200_pool* pool);
 B200_API int32_t b200_pool_num_runners(const b200_pool* pool);
 B200_API b200_runner* b200_pool_runner(b200_pool* pool, int32_t index);
@@ -454,6 +496,15 @@ B200_API int b200_modbase_runner_debug_read_workspace(b200_modbase_runner* runne
  * = (y, gate)): c = E4M3 [M,N/2] of y * silu(gate). */
 B200_API int b200_test_gemm_fp8(int32_t device, const uint8_t* a, const uint8_t* b, int32_t M, int32_t N, int32_t K,
                                 int32_t activation, const uint16_t* residual, float alpha, void* c);
+/* The GEMM with int8 operands (A [M,K], W [N,K]; K is zero-padded to a multiple of 128 inside):
+ * c = act(float(A W^T) * col_scale[n] + bias[n]) as fp16 [M,N]; the s32 accumulation is exact.  activation -1 or 3 (tanh x 5);
+ * bias may be NULL. */
+B200_API int b200_test_gemm_s8(int32_t device, const int8_t* a, const int8_t* b, const float* col_scale, const float* bias,
+                               int32_t M, int32_t N, int32_t K, int32_t activation, uint16_t* c);
+/* Host only, no device: the int8_lstm weight quantisation of fp16 values [rows, cols], per row, as utils::quantize_tensor(w, 1)
+ * computes it on an fp16 tensor: scale = fp16(128 / absmax), q = clip(round_half_even(fp16(w * scale)), -127, 127).  An all-zero
+ * row gets q = 0 and scale = +inf (the engine dequantises such a row with the factor 0). */
+B200_API int b200_test_quantize_rows(const uint16_t* f16, int32_t rows, int32_t cols, int8_t* q, uint16_t* scale);
 /* Host only, no device: the fp8_ffn weight rounding.  to_e4m3: torch's float8_e4m3fn cast of each fp16 value (round to
  * nearest even; NaN beyond the range).  remove_bits: the reference's (bits + 2^(b-1)) & ~(2^b - 1) on the int16 view. */
 B200_API int b200_test_to_e4m3(const uint16_t* f16, int64_t n, uint8_t* out);
