@@ -406,6 +406,13 @@ int b200_test_gemm(int32_t device, const uint16_t* a, const uint16_t* b, const f
     });
 }
 
+int b200_test_gemm_desc(int32_t device, const b200_gemm_test_desc* desc) {
+    return guarded([&] {
+        if (!desc) throw std::invalid_argument("b200_test_gemm_desc: null argument");
+        b200::test_gemm_desc_host(device, *desc);
+    });
+}
+
 int b200_test_gemm_fp8(int32_t device, const uint8_t* a, const uint8_t* b, int32_t M, int32_t N, int32_t K, int32_t activation,
                        const uint16_t* residual, float alpha, void* c) {
     return guarded([&] {

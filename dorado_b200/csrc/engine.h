@@ -374,6 +374,9 @@ void decode_host_scores(int device, const uint16_t* scores, int N, int T, int C,
                         int32_t* n_bases);
 void test_gemm_host(int device, const uint16_t* a, const uint16_t* b, const float* bias, int M, int N, int K,
                     int activation, uint16_t* c);
+void test_gemm_desc_host(int device, const b200_gemm_test_desc& t);
+// The transformer's rotary table (tx_model.cu): [16 dim pairs][tmax positions] float4 (cos, sin, cos, sin), in fp32
+std::vector<float> rope_table(float theta, int tmax);
 void test_attention_host(int device, const uint16_t* qkv, int N, int T, int H, int win_upper, int win_lower, uint16_t* out);
 void test_gemm_fp8_host(int device, const uint8_t* a, const uint8_t* b, int M, int N, int K, int activation,
                         const uint16_t* residual, float alpha, void* c);

@@ -21,8 +21,10 @@
 #include "common.cuh"
 #include "engine.h"
 
+#include <algorithm>
 #include <cstdlib>
 #include <cstring>
+#include <string>
 #include <type_traits>
 #include <vector>
 
@@ -46,9 +48,6 @@ struct GemmKernelParams {
     __half* out;
     uint32_t out_m1;
     long long out_s0, out_s1;
-    uint32_t out_col_m1;
-    long long out_col_s0;
-    int bias_per_row;
     const float* rope;
     int rope_T, rope_cols, rope_stride;
     const __half* residual;
@@ -202,10 +201,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
         const int r0 = (mt % p.tiles_per_batch) * BM;
         const int n0 = nt * p.bn;
         // 32-bit division only: a 64-bit division is a library call, and a call in this function makes ptxas serialise the
-        // wgmma pipeline.  make_gemm_plan checks that rows, strides and column blocking fit in 32 bits.
+        // wgmma pipeline.  make_gemm_plan checks that rows and the output blocking fit in 32 bits.
         bool valid[2];
         long long g[2], off[2];
-        float r_a[2], r_res[2], row_bias[2];
+        float r_a[2], r_res[2];
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int row = r0 + rloc + 8 * h;
@@ -226,7 +225,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                 for (int i = 0; i < p.res_ss_parts; ++i) ss += __ldg(p.res_ss + g[h] * p.res_ss_parts + i);
                 r_res[h] = rsqrtf(ss * p.norm_inv_dim + p.norm_eps);
             }
-            row_bias[h] = (p.bias && p.bias_per_row && valid[h]) ? __ldg(p.bias + g[h]) : 0.0f;
         }
         if constexpr (S8) {
             // s32 -> fp32 is exact for the K this form is used at (|acc| <= 127^2 K < 2^24 up to K = 1024)
@@ -286,17 +284,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                 for (int j = 0; j < 4; ++j) {
                     const int nc = n0 + c * 32 + 8 * j + 2 * quad;
                     float2 b2 = make_float2(0.0f, 0.0f);
-                    if (p.bias && !p.bias_per_row) b2 = __ldg(reinterpret_cast<const float2*>(p.bias + nc));
+                    if (p.bias) b2 = __ldg(reinterpret_cast<const float2*>(p.bias + nc));
                     float2 gain = make_float2(1.0f, 1.0f);
                     if (p.residual && p.res_gain) gain = __ldg(reinterpret_cast<const float2*>(p.res_gain + nc));
-                    const long long coff = p.out_col_m1 > 0
-                            ? (long long)((uint32_t)nc / p.out_col_m1) * p.out_col_s0 + (long long)((uint32_t)nc % p.out_col_m1)
-                            : nc;
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         if (!valid[h]) continue;
-                        float v0 = acc[c][4 * j + 2 * h] * r_a[h] + b2.x + row_bias[h];
-                        float v1 = acc[c][4 * j + 2 * h + 1] * r_a[h] + b2.y + row_bias[h];
+                        float v0 = acc[c][4 * j + 2 * h] * r_a[h] + b2.x;
+                        float v1 = acc[c][4 * j + 2 * h + 1] * r_a[h] + b2.y;
                         if constexpr (ACT == GEMM_ACT_SWIGLU) {
                             // columns (2i, 2i + 1) = (y, gate) -> output column i
                             if constexpr (FP8) {
@@ -321,10 +316,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                             if constexpr (Q8 == GEMM_Q8_STORE) {
                                 const int32_t q0 = tc::cvt_rni_sat_s8(kInt8ActScale * act_apply<ACT>(v0));
                                 const int32_t q1 = tc::cvt_rni_sat_s8(kInt8ActScale * act_apply<ACT>(v1));
-                                *reinterpret_cast<uint16_t*>(reinterpret_cast<int8_t*>(p.out) + off[h] + coff) =
+                                *reinterpret_cast<uint16_t*>(reinterpret_cast<int8_t*>(p.out) + off[h] + nc) =
                                         (uint16_t)((q0 & 0xff) | ((q1 & 0xff) << 8));
                             } else {
-                                *reinterpret_cast<__half2*>(p.out + off[h] + coff) = o;
+                                *reinterpret_cast<__half2*>(p.out + off[h] + nc) = o;
                             }
                         }
                     }
@@ -423,7 +418,7 @@ GemmPlan make_gemm_plan(const GemmDesc& d) {
         throw std::invalid_argument(eb == 1 ? "gemm: E4M3 / int8 K must be a positive multiple of 128" : "gemm: K must be a positive multiple of 64");
     }
     if (d.q8 != GEMM_Q8_NONE) {
-        const bool plain = !d.fp8 && !d.residual && !d.out_ss && !d.a_ss && !d.res_ss && !d.bias_per_row && d.out_col_m1 == 0;
+        const bool plain = !d.fp8 && !d.residual && !d.out_ss && !d.a_ss && !d.res_ss;
         if (s8 && !(plain && d.col_scale && (d.act == GEMM_ACT_NONE || d.act == GEMM_ACT_TANH_X5))) {
             throw std::invalid_argument("gemm: int8 operands take col_scale, a column bias and the plain or TANH_X5 epilogue only");
         }
@@ -443,8 +438,10 @@ GemmPlan make_gemm_plan(const GemmDesc& d) {
     GemmPlan p{};
     p.d = d;
     p.bn = pick_bn(d.N);
-    if (d.N / p.bn < 2 && d.N >= 128 && (long long)d.batches * ((d.rows_per_batch + BM - 1) / BM) < kNumSMs / 2) {
-        p.bn = pick_bn(d.N / 2);  // few row tiles: split N further to fill more SMs
+    // few row tiles: split N further to fill more SMs.  Not with out_ss, whose partial slots are laid out for tiles of
+    // pick_bn(N) columns (gemm_out_ss_parts); the tile width only changes the occupancy.
+    if (!d.out_ss && d.N / p.bn < 2 && d.N >= 128 && (long long)d.batches * ((d.rows_per_batch + BM - 1) / BM) < kNumSMs / 2) {
+        p.bn = pick_bn(d.N / 2);
     }
     if (p.bn == 0) throw std::invalid_argument("gemm: no valid tile width");
     if (d.out_ss) {
@@ -461,8 +458,7 @@ GemmPlan make_gemm_plan(const GemmDesc& d) {
         throw std::invalid_argument("gemm: rope epilogue needs BN % 64 == 0 and a table");
     }
     p.tiles_per_batch = (d.rows_per_batch + BM - 1) / BM;
-    if ((long long)p.tiles_per_batch * BM * d.batches >= (1LL << 31) || d.out_m1 < 1 || d.out_m1 >= (1LL << 32) ||
-        d.out_col_m1 < 0 || d.out_col_m1 >= (1LL << 32)) {
+    if ((long long)p.tiles_per_batch * BM * d.batches >= (1LL << 31) || d.out_m1 < 1 || d.out_m1 >= (1LL << 32)) {
         throw std::invalid_argument("gemm: rows and output blocking must fit 32-bit index arithmetic");
     }
     p.grid = dim3((unsigned)(p.tiles_per_batch * d.batches), (unsigned)(d.N / p.bn), 1);
@@ -494,9 +490,6 @@ void run_gemm(const GemmPlan& p, cudaStream_t stream) {
     k.out_m1 = (uint32_t)p.d.out_m1;
     k.out_s0 = p.d.out_s0;
     k.out_s1 = p.d.out_s1;
-    k.out_col_m1 = (uint32_t)p.d.out_col_m1;
-    k.out_col_s0 = p.d.out_col_s0;
-    k.bias_per_row = p.d.bias_per_row;
     k.rope = p.d.rope;
     k.rope_T = p.d.rope_T;
     k.rope_cols = p.d.rope_cols;
@@ -545,46 +538,160 @@ void run_gemm(const GemmPlan& p, cudaStream_t stream) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// test hook: host buffers in, host buffer out
+// test hooks: host buffers in, host buffer out
 // ------------------------------------------------------------------------------------------------
-void test_gemm_host(int device, const uint16_t* a, const uint16_t* b, const float* bias, int M, int N, int K, int activation,
-                    uint16_t* c) {
+namespace {
+
+// Refuses, before anything is allocated, a descriptor that would make the kernel read or write outside a buffer of the
+// lengths given (b200_gemm_test_desc).  Ranges first: with rows < 2^31 and strides and offsets < 2^30, every sum below
+// stays under 2^62.
+void check_gemm_test_desc(const b200_gemm_test_desc& t) {
+    auto need = [](bool ok, const char* what) {
+        if (!ok) throw std::invalid_argument(std::string("b200_test_gemm_desc: ") + what);
+    };
+    constexpr int64_t kMax = 1LL << 30;
+    need(t.batches >= 1 && t.rows_per_batch >= 1 && (int64_t)t.batches * t.rows_per_batch < (1LL << 31), "rows out of range");
+    need(t.K >= 1 && t.K <= (1 << 16) && t.N >= 1 && t.N <= (1 << 16), "K or N out of range");
+    need(t.a_inner >= 0 && t.a_inner <= t.K, "a_inner must lie in [0, K]");
+    need(t.a_row_stride >= 0 && t.a_row_stride < kMax && t.a_batch_stride >= 0 && t.a_batch_stride < kMax, "A strides out of range");
+    need(t.out_offset >= 0 && t.out_offset < kMax && t.out_m1 >= 1 && t.out_m1 < kMax && t.out_s0 >= 0 && t.out_s0 < kMax &&
+                 t.out_s1 >= 0 && t.out_s1 < kMax, "output addressing out of range");
+    // the epilogue stores column pairs as one 4-byte __half2
+    need(t.out_offset % 2 == 0 && t.out_s0 % 2 == 0 && t.out_s1 % 2 == 0, "output offset and strides must be even");
+    need(t.a_ss_parts >= 0 && t.a_ss_parts <= 4096 && t.res_ss_parts >= 0 && t.res_ss_parts <= 4096, "partial counts out of range");
+    need(t.a_len >= 0 && t.w_len >= 0 && t.bias_len >= 0 && t.residual_len >= 0 && t.res_gain_len >= 0 && t.a_ss_len >= 0 &&
+                 t.res_ss_len >= 0 && t.out_len >= 0 && t.out_ss_len >= 0, "negative buffer length");
+    need(t.a && t.w && t.out, "A, W and out are required");
+    const int64_t rows = (int64_t)t.batches * t.rows_per_batch;
+    // A: the tensor map's extent, (a_inner or K) x rows_per_batch x batches; TMA reads nothing beyond it
+    const int64_t inner = t.a_inner > 0 ? t.a_inner : t.K;
+    need((t.batches - 1) * t.a_batch_stride + (int64_t)(t.rows_per_batch - 1) * t.a_row_stride + inner <= t.a_len, "A is too short");
+    need((int64_t)t.N * t.K <= t.w_len, "W is too short");
+    need(!t.bias || t.N <= t.bias_len, "bias is too short");
+    // out: the largest row offset over g < rows, with non-negative strides at the last g or at the last g of the previous
+    // out_m1 block
+    const int64_t q = (rows - 1) / t.out_m1, r = (rows - 1) % t.out_m1;
+    int64_t last_row = q * t.out_s0 + r * t.out_s1;
+    if (q > 0) last_row = std::max(last_row, (q - 1) * t.out_s0 + (t.out_m1 - 1) * t.out_s1);
+    const int n_out = t.act == GEMM_ACT_SWIGLU ? t.N / 2 : t.N;
+    need(t.out_offset + last_row + n_out <= t.out_len, "out is too short");
+    // the residual is addressed as g * N + n whatever the output strides
+    need(!t.residual || rows * t.N <= t.residual_len, "residual is too short");
+    need(!t.res_gain || t.N <= t.res_gain_len, "res_gain is too short");
+    need(!t.a_ss || rows * t.a_ss_parts <= t.a_ss_len, "a_ss is too short");
+    need(!t.res_ss || rows * t.res_ss_parts <= t.res_ss_len, "res_ss is too short");
+    need(!t.out_ss || rows * (t.N / 32) <= t.out_ss_len, "out_ss is too short");
+    if (t.act == GEMM_ACT_ROPE) {
+        // the table has max_seq_len positions per dim pair, and the kernel reads position g % rope_T
+        need(t.theta > 0.0f && t.max_seq_len >= 1 && t.max_seq_len <= (1 << 16) && t.rope_T >= 1 && t.rope_T <= t.max_seq_len,
+             "RoPE needs theta > 0 and 1 <= rope_T <= max_seq_len");
+    }
+}
+
+}  // namespace
+
+void test_gemm_desc_host(int device, const b200_gemm_test_desc& t) {
+    check_gemm_test_desc(t);
     require_sm90(device);
-    const int Kp = (K + BK - 1) / BK * BK;
-    const int n_out = activation == GEMM_ACT_SWIGLU ? N / 2 : N;
-    __half *d_a = nullptr, *d_w = nullptr, *d_c = nullptr;
-    float* d_bias = nullptr;
+    const int64_t rows = (int64_t)t.batches * t.rows_per_batch;
+    const std::vector<float> rope = t.act == GEMM_ACT_ROPE ? rope_table(t.theta, t.max_seq_len) : std::vector<float>();
+    auto bytes = [](int64_t n, size_t elem) { return (size_t)(n > 0 ? n : 1) * elem; };
+    __half *d_a = nullptr, *d_w = nullptr, *d_res = nullptr, *d_out = nullptr;
+    float *d_bias = nullptr, *d_gain = nullptr, *d_a_ss = nullptr, *d_res_ss = nullptr, *d_out_ss = nullptr, *d_rope = nullptr;
     Arena arena;
     arena.allocate([&](Bump& b) {
-        d_a = b.take<__half>((size_t)M * Kp * 2);
-        d_w = b.take<__half>((size_t)N * Kp * 2);
-        d_bias = b.take<float>((size_t)N * 4);
-        d_c = b.take<__half>((size_t)M * n_out * 2);
+        d_a = b.take<__half>(bytes(t.a_len, 2));
+        d_w = b.take<__half>(bytes(t.w_len, 2));
+        d_bias = b.take<float>(bytes(t.bias_len, 4));
+        d_res = b.take<__half>(bytes(t.residual_len, 2));
+        d_gain = b.take<float>(bytes(t.res_gain_len, 4));
+        d_a_ss = b.take<float>(bytes(t.a_ss_len, 4));
+        d_res_ss = b.take<float>(bytes(t.res_ss_len, 4));
+        d_out = b.take<__half>(bytes(t.out_len, 2));
+        d_out_ss = b.take<float>(bytes(t.out_ss_len, 4));
+        d_rope = b.take<float>(bytes((int64_t)rope.size(), 4));
     });
-    B200_CUDA(cudaMemset(d_a, 0, (size_t)M * Kp * 2));
-    B200_CUDA(cudaMemset(d_w, 0, (size_t)N * Kp * 2));
-    B200_CUDA(cudaMemcpy2D(d_a, (size_t)Kp * 2, a, (size_t)K * 2, (size_t)K * 2, M, cudaMemcpyHostToDevice));
-    B200_CUDA(cudaMemcpy2D(d_w, (size_t)Kp * 2, b, (size_t)K * 2, (size_t)K * 2, N, cudaMemcpyHostToDevice));
-    if (bias) B200_CUDA(cudaMemcpy(d_bias, bias, (size_t)N * 4, cudaMemcpyHostToDevice));
+    auto up = [](void* dst, const void* src, int64_t n, size_t elem) {
+        if (src && n > 0) B200_CUDA(cudaMemcpy(dst, src, (size_t)n * elem, cudaMemcpyHostToDevice));
+    };
+    up(d_a, t.a, t.a_len, 2);
+    up(d_w, t.w, t.w_len, 2);
+    up(d_bias, t.bias, t.bias_len, 4);
+    up(d_res, t.residual, t.residual_len, 2);
+    up(d_gain, t.res_gain, t.res_gain_len, 4);
+    up(d_a_ss, t.a_ss, t.a_ss_len, 4);
+    up(d_res_ss, t.res_ss, t.res_ss_len, 4);
+    up(d_out, t.out, t.out_len, 2);
+    up(d_rope, rope.data(), (int64_t)rope.size(), 4);
+    if (t.out_ss) B200_CUDA(cudaMemset(d_out_ss, 0xff, bytes(t.out_ss_len, 4)));   // NaN: a partial never written shows
     GemmDesc d{};
     d.a = d_a;
-    d.batches = 1;
-    d.rows_per_batch = M;
-    d.a_row_stride = Kp;
-    d.a_batch_stride = (int64_t)M * Kp;
+    d.batches = t.batches;
+    d.rows_per_batch = t.rows_per_batch;
+    d.a_row_stride = t.a_row_stride;
+    d.a_batch_stride = t.a_batch_stride;
+    d.a_inner = t.a_inner;
     d.w = d_w;
-    d.N = N;
-    d.K = Kp;
-    d.bias = bias ? d_bias : nullptr;
-    d.act = activation;
-    d.out = d_c;
-    d.out_m1 = 1;
-    d.out_s0 = n_out;
-    d.out_s1 = 0;
+    d.N = t.N;
+    d.K = t.K;
+    d.bias = t.bias ? d_bias : nullptr;
+    d.act = t.act;
+    d.out = d_out + t.out_offset;
+    d.out_m1 = t.out_m1;
+    d.out_s0 = t.out_s0;
+    d.out_s1 = t.out_s1;
+    if (t.act == GEMM_ACT_ROPE) {
+        d.rope = d_rope;
+        d.rope_T = t.rope_T;
+        d.rope_cols = t.rope_cols;
+        d.rope_stride = t.max_seq_len;
+    }
+    d.max_ctas = t.max_ctas;
+    d.residual = t.residual ? d_res : nullptr;
+    d.alpha = t.alpha;
+    d.out_ss = t.out_ss ? d_out_ss : nullptr;
+    d.a_ss = t.a_ss ? d_a_ss : nullptr;
+    d.a_ss_parts = t.a_ss_parts;
+    d.res_ss = t.res_ss ? d_res_ss : nullptr;
+    d.res_ss_parts = t.res_ss_parts;
+    d.res_gain = t.res_gain ? d_gain : nullptr;
+    d.norm_dim = t.norm_dim;
+    d.norm_eps = t.norm_eps;
     const GemmPlan plan = make_gemm_plan(d);
     run_gemm(plan, nullptr);
     B200_CUDA(cudaDeviceSynchronize());
-    B200_CUDA(cudaMemcpy(c, d_c, (size_t)M * n_out * 2, cudaMemcpyDeviceToHost));
+    B200_CUDA(cudaMemcpy(t.out, d_out, (size_t)t.out_len * 2, cudaMemcpyDeviceToHost));
+    if (t.out_ss) B200_CUDA(cudaMemcpy(t.out_ss, d_out_ss, (size_t)rows * (t.N / 32) * 4, cudaMemcpyDeviceToHost));
+}
+
+// The dense form: A [M][K], W [N][K], K zero-padded to a multiple of 64 here, c [M][N] (N / 2 with SwiGLU)
+void test_gemm_host(int device, const uint16_t* a, const uint16_t* b, const float* bias, int M, int N, int K, int activation,
+                    uint16_t* c) {
+    if (M < 1 || N < 1 || K < 1) throw std::invalid_argument("test_gemm: empty operand");
+    const int Kp = (K + BK - 1) / BK * BK;
+    const int n_out = activation == GEMM_ACT_SWIGLU ? N / 2 : N;
+    std::vector<uint16_t> ap((size_t)M * Kp, 0), wp((size_t)N * Kp, 0);
+    for (int m = 0; m < M; ++m) std::memcpy(&ap[(size_t)m * Kp], a + (size_t)m * K, (size_t)K * 2);
+    for (int n = 0; n < N; ++n) std::memcpy(&wp[(size_t)n * Kp], b + (size_t)n * K, (size_t)K * 2);
+    b200_gemm_test_desc t{};
+    t.a = ap.data();
+    t.a_len = (int64_t)ap.size();
+    t.w = wp.data();
+    t.w_len = (int64_t)wp.size();
+    t.bias = bias;
+    t.bias_len = bias ? N : 0;
+    t.out = c;
+    t.out_len = (int64_t)M * n_out;
+    t.batches = 1;
+    t.rows_per_batch = M;
+    t.a_row_stride = Kp;
+    t.a_batch_stride = (int64_t)M * Kp;
+    t.K = Kp;
+    t.N = N;
+    t.act = activation;
+    t.out_m1 = 1;
+    t.out_s0 = n_out;
+    test_gemm_desc_host(device, t);
 }
 
 // E4M3 operands (A [M][K], W [N][K] bytes, K zero-padded to a multiple of 128): the plain epilogue with an optional deepnorm

@@ -54,11 +54,6 @@ struct GemmDesc {
     int64_t out_m1 = 1;
     int64_t out_s0 = 0;
     int64_t out_s1 = 0;
-    // optional column blocking of the output: column n -> (n / out_col_m1) * out_col_s0 + (n % out_col_m1)
-    // (out_col_m1 = 0: plain contiguous columns).  out_col_m1 must be a multiple of 32.
-    int64_t out_col_m1 = 0;
-    int64_t out_col_s0 = 0;
-    int bias_per_row = 0;  // bias indexed by the global row g instead of the column
     // GEMM_ACT_ROPE: (cos, sin) table [T_max][32][2], tokens per chunk, number of leading columns to rotate
     const float* rope = nullptr;
     int rope_T = 0;

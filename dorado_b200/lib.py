@@ -84,6 +84,23 @@ class ModBaseDesc(C.Structure):
                 ("kmer_len", C.c_int32), ("chunk_size", C.c_int32)]
 
 
+class GemmTestDesc(C.Structure):
+    """b200_gemm_test_desc"""
+    _fields_ = [
+        ("a", C.c_void_p), ("a_len", C.c_int64), ("w", C.c_void_p), ("w_len", C.c_int64),
+        ("bias", C.c_void_p), ("bias_len", C.c_int64), ("residual", C.c_void_p), ("residual_len", C.c_int64),
+        ("res_gain", C.c_void_p), ("res_gain_len", C.c_int64), ("a_ss", C.c_void_p), ("a_ss_len", C.c_int64),
+        ("res_ss", C.c_void_p), ("res_ss_len", C.c_int64), ("out", C.c_void_p), ("out_len", C.c_int64),
+        ("out_ss", C.c_void_p), ("out_ss_len", C.c_int64),
+        ("batches", C.c_int32), ("rows_per_batch", C.c_int32), ("a_row_stride", C.c_int64), ("a_batch_stride", C.c_int64),
+        ("a_inner", C.c_int32), ("K", C.c_int32), ("N", C.c_int32), ("act", C.c_int32),
+        ("out_offset", C.c_int64), ("out_m1", C.c_int64), ("out_s0", C.c_int64), ("out_s1", C.c_int64),
+        ("alpha", C.c_float), ("a_ss_parts", C.c_int32), ("res_ss_parts", C.c_int32), ("norm_dim", C.c_int32),
+        ("norm_eps", C.c_float), ("max_ctas", C.c_int32), ("theta", C.c_float),
+        ("max_seq_len", C.c_int32), ("rope_T", C.c_int32), ("rope_cols", C.c_int32),
+    ]
+
+
 class Stats(C.Structure):
     _fields_ = [("batches_called", C.c_int64), ("model_decode_ms", C.c_double), ("h2d_ms", C.c_double),
                 ("d2h_ms", C.c_double), ("gpu_launches", C.c_int64), ("arena_bytes", C.c_int64)]
@@ -95,7 +112,7 @@ EXPORTS = [
     "b200_runner_set_decoder_options", "b200_runner_batch_size", "b200_runner_chunk_size", "b200_runner_out_len",
     "b200_runner_accept_chunk_f16", "b200_runner_accept_chunk_f32", "b200_runner_input", "b200_runner_call_chunks",
     "b200_runner_upload", "b200_runner_step_device", "b200_runners_step_device", "b200_runner_forward_scores", "b200_runner_profile", "b200_runner_plan_info", "b200_runner_debug_read_workspace", "b200_decode_scores",
-    "b200_test_gemm", "b200_test_gemm_fp8", "b200_test_gemm_s8", "b200_test_quantize_rows", "b200_test_to_e4m3", "b200_test_remove_bits", "b200_test_attention", "b200_generate_chunks", "b200_stitch_chunks", "b200_runner_accept_raw_chunk",
+    "b200_test_gemm", "b200_test_gemm_desc", "b200_test_gemm_fp8", "b200_test_gemm_s8", "b200_test_quantize_rows", "b200_test_to_e4m3", "b200_test_remove_bits", "b200_test_attention", "b200_generate_chunks", "b200_stitch_chunks", "b200_runner_accept_raw_chunk",
     "b200_runner_debug_read_input", "b200_engine_runner_bytes", "b200_engine_benchmark_batch_sizes",
     "b200_select_batch_size", "b200_generate_variable_chunks", "b200_engine_terminate", "b200_engine_restart",
     "b200_engine_set_low_latency", "b200_engine_is_low_latency", "b200_engine_batch_timeouts_ms",
@@ -179,6 +196,7 @@ def load_library() -> C.CDLL:
     lib.b200_runner_plan_info.argtypes = [vp, C.c_char_p, C.c_uint64]
     lib.b200_runner_debug_read_workspace.argtypes = [vp, C.c_uint64, C.c_uint64, vp]
     lib.b200_test_gemm.argtypes = [i32, vp, vp, vp, i32, i32, i32, i32, vp]
+    lib.b200_test_gemm_desc.argtypes = [i32, C.POINTER(GemmTestDesc)]
     lib.b200_test_attention.argtypes = [i32, vp, i32, i32, i32, i32, i32, vp]
     lib.b200_test_gemm_fp8.argtypes = [i32, vp, vp, i32, i32, i32, i32, vp, f32, vp]
     lib.b200_test_gemm_s8.argtypes = [i32, vp, vp, vp, vp, i32, i32, i32, i32, vp]
@@ -291,6 +309,37 @@ def test_gemm(a: np.ndarray, b: np.ndarray, bias: np.ndarray | None, activation:
         bias_p = bias.ctypes.data
     check(lib.b200_test_gemm(device, a.ctypes.data, b.ctypes.data, bias_p, M, N, K, activation, c.ctypes.data))
     return c
+
+
+def test_gemm_desc(a: np.ndarray, w: np.ndarray, out: np.ndarray, *, rows_per_batch: int, a_row_stride: int, out_s0: int,
+                   batches: int = 1, a_batch_stride: int = 0, a_inner: int = 0, act: int = -1, out_offset: int = 0,
+                   out_m1: int = 1, out_s1: int = 0, bias=None, residual=None, alpha: float = 0.0, res_gain=None,
+                   a_ss=None, a_ss_parts: int = 0, res_ss=None, res_ss_parts: int = 0, norm_dim: int = 0,
+                   norm_eps: float = 1e-5, max_ctas: int = 0, theta: float = 0.0, max_seq_len: int = 0, rope_T: int = 0,
+                   rope_cols: int = 0, out_ss: bool = False, device: int = 0):
+    """The fp16 GEMM launched from a full descriptor (b200_test_gemm_desc): a is any flat fp16 buffer, w [N, K] fp16, out the
+    whole output buffer with the caller's sentinel in it.  Returns (the output buffer after the GEMM, the [rows, N / 32]
+    partial sums of squares or None)."""
+    lib = load_library()
+    flat = lambda x, t: None if x is None else np.ascontiguousarray(np.ravel(x), t)
+    a, res, outb = flat(a, np.float16), flat(residual, np.float16), flat(out, np.float16).copy()
+    w = np.ascontiguousarray(w, np.float16)
+    bias, res_gain, a_ss, res_ss = (flat(x, np.float32) for x in (bias, res_gain, a_ss, res_ss))
+    N, K = w.shape
+    ss = np.empty((batches * rows_per_batch, N // 32), np.float32) if out_ss else None
+    d = GemmTestDesc()
+    for name, arr in (("a", a), ("w", w), ("bias", bias), ("residual", res), ("res_gain", res_gain), ("a_ss", a_ss),
+                      ("res_ss", res_ss), ("out", outb), ("out_ss", ss)):
+        if arr is not None:
+            setattr(d, name, arr.ctypes.data)
+            setattr(d, name + "_len", arr.size)
+    d.batches, d.rows_per_batch, d.a_row_stride, d.a_batch_stride = batches, rows_per_batch, a_row_stride, a_batch_stride
+    d.a_inner, d.K, d.N, d.act = a_inner, K, N, act
+    d.out_offset, d.out_m1, d.out_s0, d.out_s1 = out_offset, out_m1, out_s0, out_s1
+    d.alpha, d.a_ss_parts, d.res_ss_parts, d.norm_dim, d.norm_eps = alpha, a_ss_parts, res_ss_parts, norm_dim, norm_eps
+    d.max_ctas, d.theta, d.max_seq_len, d.rope_T, d.rope_cols = max_ctas, theta, max_seq_len, rope_T, rope_cols
+    check(lib.b200_test_gemm_desc(device, C.byref(d)))
+    return outb, ss
 
 
 def test_gemm_fp8(a: np.ndarray, b: np.ndarray, activation: int = -1, residual: np.ndarray | None = None,

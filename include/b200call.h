@@ -512,6 +512,36 @@ B200_API int b200_test_remove_bits(const uint16_t* f16, int64_t n, int32_t bits,
 B200_API int b200_test_gemm(int32_t device, const uint16_t* a /* [M,K] fp16 */, const uint16_t* b /* [N,K] fp16 */,
                             const float* bias /* [N] or NULL */, int32_t M, int32_t N, int32_t K, int32_t activation,
                             uint16_t* c /* [M,N] fp16 */);
+/* The fp16 GEMM launched from every field the model plans set (dorado_b200/csrc/gemm.h, GemmDesc), on host buffers.  Each
+ * buffer comes with its length in elements; a descriptor that would read or write beyond one returns B200_ERR_INVALID
+ * before anything is allocated.  Rows g = batch * rows_per_batch + r, r < rows_per_batch, read A at
+ * batch * a_batch_stride + r * a_row_stride + k for k < (a_inner ? a_inner : K) (zeros beyond, up to K) and write
+ * out + out_offset + (g / out_m1) * out_s0 + (g % out_m1) * out_s1 + n for n < N (N / 2 with SwiGLU).  The residual is
+ * read at g * N + n, the partial sums of squares at g * parts + i.  out holds the caller's sentinel on entry and the
+ * whole buffer on return.  out_ss, when not NULL, receives the N / 32 partials of every row (NaN where none was written).
+ * act 5 (RoPE) takes the model's own table for theta and max_seq_len, and rotates position g % rope_T. */
+typedef struct b200_gemm_test_desc {
+    const uint16_t* a;         int64_t a_len;         /* fp16, flat: overlapping and padded views are the caller's */
+    const uint16_t* w;         int64_t w_len;         /* fp16 [N][K] */
+    const float* bias;         int64_t bias_len;      /* [N] or NULL */
+    const uint16_t* residual;  int64_t residual_len;  /* fp16 or NULL */
+    const float* res_gain;     int64_t res_gain_len;  /* [N] or NULL */
+    const float* a_ss;         int64_t a_ss_len;      /* [rows][a_ss_parts] or NULL */
+    const float* res_ss;       int64_t res_ss_len;    /* [rows][res_ss_parts] or NULL */
+    uint16_t* out;             int64_t out_len;       /* fp16 */
+    float* out_ss;             int64_t out_ss_len;    /* [rows][N / 32] or NULL */
+    int32_t batches, rows_per_batch;
+    int64_t a_row_stride, a_batch_stride;
+    int32_t a_inner, K, N, act;
+    int64_t out_offset, out_m1, out_s0, out_s1;
+    float alpha;
+    int32_t a_ss_parts, res_ss_parts, norm_dim;
+    float norm_eps;
+    int32_t max_ctas;
+    float theta;
+    int32_t max_seq_len, rope_T, rope_cols;
+} b200_gemm_test_desc;
+B200_API int b200_test_gemm_desc(int32_t device, const b200_gemm_test_desc* desc);
 /* The transformer's sliding-window attention kernel, launched exactly as the model launches it: qkv of N chunks of T tokens
  * (q and k already rotated), query i of a chunk attends keys j with -win_upper <= j - i <= win_lower, softmax scale 1/8.
  * Windows outside [0, 256] return B200_ERR_UNSUPPORTED. */
