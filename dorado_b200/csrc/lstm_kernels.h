@@ -57,7 +57,7 @@ struct LstmStackDesc {
     int runners = 1;             // batches in flight: sizes the grid recurrence and caps the x-projection GEMM's CTAs
     bool reverse_first = false;  // layer 0 (and every other layer after it) runs reversed in time
     // int8 layers (lstm_size 256 and 384): seq holds int8 cvt.rni.sat.s8(kInt8ActScale * v), the x-projection and the
-    // recurrence run on int8 operands with s32 accumulation (lstm_rec_i8_kernel), gx stays fp16
+    // recurrence run on int8 operands with s32 accumulation (the int8 form of lstm_rec_kernel), gx stays fp16
     bool int8 = false;
     void* seq = nullptr;         // [T + 1][Np][C] fp16 (int8 if `int8`): the first layer's input, overwritten in place with h by every layer
     const LstmLayerWeights* layers = nullptr;  // kept by the caller for the stack's lifetime
@@ -76,7 +76,7 @@ LstmStackBuffers carve_lstm_stack(Bump& b, int C, int num_layers, int T, int Np)
 
 // Every layer is lstm_layer_kernel (lstm_size 96), or the x-projection GEMM followed by lstm_rec_kernel (128 - 384) or by
 // one or more cooperative launches of lstm_grid_rec_kernel (768, 1024); int8 layers are the int8 x-projection GEMM followed
-// by lstm_rec_i8_kernel.  Built once per batch shape; reads
+// by the int8 form of lstm_rec_kernel.  Built once per batch shape; reads
 // B200_DEBUG_LSTM_LAYERS, B200_CLUSTER_CHUNKS, B200_GRID_CHUNKS and B200_GRID_GROUPS then.
 class LstmStack {
 public:

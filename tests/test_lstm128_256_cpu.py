@@ -3,8 +3,8 @@ model of how lstm_rec_kernel (dorado_b200/csrc/lstm_model.cu) partitions the rec
 these widths.  The GPU side is tests/test_lstm128_256_gpu.py, which also pins the launch-shape model below to the plan
 the library builds.
 
-Both widths run the x-projection GEMM followed by lstm_rec_kernel<C, CL, NB>, with CL = rec_cluster(C): 4 CTAs for 128,
-8 for 256, so every CTA owns U = 32 hidden units (128 gate rows, 8 warps)."""
+Both widths run the x-projection GEMM followed by the fp16 form lstm_rec_kernel<false, C, CL, NB>, with
+CL = rec_cluster(C): 4 CTAs for 128, 8 for 256, so every CTA owns U = 32 hidden units (128 gate rows, 8 warps)."""
 import pathlib
 import re
 
@@ -33,25 +33,27 @@ def rec_cluster(C):
 
 
 class RecCfg:
-    """lstm_model.cu RecCfg<C, CL, NB>, with its static_asserts."""
+    """lstm_model.cu RecCfg<I8, C, CL, NB>, with its static_asserts; the fp16 form unless i8."""
 
-    def __init__(self, C, CL, NB):
+    def __init__(self, C, CL, NB, i8=False):
         self.C, self.CL, self.NB = C, CL, NB
+        self.EB = 1 if i8 else 2          # bytes per element of W_hh and h
         self.U = C // CL
         self.MT = 4 * self.U // 16
         self.THREADS = 32 * self.MT
-        self.KS = C // 16
+        self.KE = 32 // self.EB
+        self.KS = C // self.KE
         self.NT = NB // 8
-        self.HS = C + 8
+        self.HS = C + 16 // self.EB
         self.GS = NB + 4
         self.PAIRS = self.U // 2 * NB // self.THREADS
         self.GX_AHEAD = self.PAIRS <= 2
-        self.SMEM = 2 * NB * self.HS * 2 + 4 * self.U * self.GS * 4
+        self.SMEM = 2 * NB * self.HS * self.EB + 4 * self.U * self.GS * 4
 
     def static_asserts_hold(self):
-        shape = (self.C % self.CL == 0 and self.U % 4 == 0 and self.NT % 2 == 0 and self.PAIRS >= 1
-                 and (self.U // 2 * self.NB) % self.THREADS == 0)
-        return shape and self.THREADS <= 1024 and 1 < self.CL <= 8
+        shape = (self.C % self.KE == 0 and self.C % self.CL == 0 and self.U % 4 == 0 and self.NT % 2 == 0
+                 and self.PAIRS >= 1 and (self.U // 2 * self.NB) % self.THREADS == 0)
+        return shape and self.HS * self.EB % 128 == 16 and self.THREADS <= 1024 and 1 < self.CL <= 8
 
 
 def lstm_rec_chunks(Np, override=None):
@@ -142,6 +144,11 @@ def test_rec_cfg(C, NB):
     assert cfg.SMEM <= MAX_SMEM
     # 4 KS A-fragment registers per thread hold W_hh: 32 for 128, 64 for 256
     assert 4 * cfg.KS == C // 4
+    if C == 256:   # the int8 form: the same partition and gx schedule, half the K steps, h rows of C + 16 bytes
+        i8 = RecCfg(C, rec_cluster(C), NB, i8=True)
+        assert i8.static_asserts_hold()
+        assert (i8.THREADS, i8.PAIRS, i8.GX_AHEAD, i8.KS, i8.HS) == (cfg.THREADS, cfg.PAIRS, cfg.GX_AHEAD, C // 32, C + 16)
+        assert i8.SMEM < cfg.SMEM
 
 
 @pytest.mark.parametrize("C", [128, 256])
@@ -215,12 +222,12 @@ def test_launch_shape(C):
 
 
 def _ptxas_entries():
-    """(C, CL, NB) -> (registers, stack bytes, spill store bytes, spill load bytes) of lstm_rec_kernel from the build's
-    ptxas log."""
+    """(C, CL, NB) -> (registers, stack bytes, spill store bytes, spill load bytes) of the fp16 form of lstm_rec_kernel from
+    the build's ptxas log."""
     text = PTXAS_LOG.read_text()
     out = {}
     for block in re.split(r"ptxas info\s*: Compiling entry function ", text)[1:]:
-        m = re.match(r"'_ZN4b200\w*?15lstm_rec_kernelILi(\d+)ELi(\d+)ELi(\d+)E", block)
+        m = re.match(r"'_ZN4b200\w*?15lstm_rec_kernelILb0ELi(\d+)ELi(\d+)ELi(\d+)E", block)
         if not m:
             continue
         frame = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", block)
@@ -229,15 +236,15 @@ def _ptxas_entries():
     return out
 
 
-def test_ptxas_reports_no_spills():
-    """Every lstm_rec_kernel<128 | 256, CL, NB> of the built library: no stack frame, no spills, one CTA of 256 threads
+def test_ptxas_reports_no_spills_in_the_fp16_rec_form():
+    """Every lstm_rec_kernel<false, 128 | 256, CL, NB> of the built library: no stack frame, no spills, one CTA of 256 threads
     within the 255-register cap."""
     if not PTXAS_LOG.is_file():
         pytest.skip("dorado_b200/csrc/build/lstm_model.ptxas.log not built")
     entries = _ptxas_entries()
     for C, NB in SHAPES:
         key = (C, rec_cluster(C), NB)
-        assert key in entries, f"no lstm_rec_kernel<{C}, {key[1]}, {NB}> in the ptxas log"
+        assert key in entries, f"no lstm_rec_kernel<false, {C}, {key[1]}, {NB}> in the ptxas log"
         regs, stack, st, ld = entries[key]
         assert (stack, st, ld) == (0, 0, 0), (key, entries[key])
         assert regs <= 255

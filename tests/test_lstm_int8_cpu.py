@@ -183,7 +183,7 @@ def _entries(log, pattern):
     return out
 
 
-def test_ptxas_reports_no_spills():
+def test_ptxas_reports_no_spills_in_the_int8_kernels():
     """The int8 instantiations: no stack, no spills, within the registers one CTA per SM of their block size allows."""
     if not (BUILD / "gemm.ptxas.log").is_file() or not (BUILD / "lstm_model.ptxas.log").is_file():
         pytest.skip("the ptxas logs are not built")
@@ -193,9 +193,9 @@ def test_ptxas_reports_no_spills():
     for key, (regs, stack, st, ld) in gemm.items():
         print(f"\n[gemm_wgmma_kernel<{key}>] {regs} registers, {stack} B stack, {st} / {ld} B spills")
         assert stack == 0 and st == 0 and ld == 0 and regs * 384 <= 65536
-    rec = _entries("lstm_model.ptxas.log", r"lstm_rec_i8_kernelILi(\d+)ELi(\d+)ELi(\d+)EE")
+    rec = _entries("lstm_model.ptxas.log", r"lstm_rec_kernelILb1ELi(\d+)ELi(\d+)ELi(\d+)EE")
     assert sorted(rec) == sorted((str(c), "8", str(nb)) for c in (256, 384) for nb in (16, 32, 64))
     for (c, cl, nb), (regs, stack, st, ld) in sorted(rec.items()):
         threads = 32 * (4 * int(c) // int(cl)) // 16
-        print(f"[lstm_rec_i8_kernel<{c}, {cl}, {nb}>] {regs} registers, {stack} B stack, {st} / {ld} B spills")
+        print(f"[lstm_rec_kernel<true, {c}, {cl}, {nb}>] {regs} registers, {stack} B stack, {st} / {ld} B spills")
         assert stack == 0 and st == 0 and ld == 0 and regs * threads <= 65536
