@@ -394,6 +394,7 @@ public:
     int N = 0, T = 0, H = 0;
     int norm_dim = 0;   // d_model: row width of the separate RMSNorm pass
     int n_launches = 0;
+    int stop_after = -1;        // B200_DEBUG_TX_LAUNCHES: run() returns after this many launches (-1: the whole plan)
     bool fold_norm = true;
     bool fp8 = false;           // fp8_ffn: explicit norm1 pass writing fp16 (norm_out) and E4M3 (norm_out8), E4M3 fc1 / fc2
     __half* norm_out = nullptr;
@@ -751,75 +752,88 @@ std::unique_ptr<ForwardPlan> TxModel::make_plan(int N, int T_in, const __half* s
     plan->norm_out = att;
     plan->norm_out8 = reinterpret_cast<uint8_t*>(qkv);
     plan->n_launches = 1 + (desc.num_convs - 1) + desc.depth * (fp8 ? 6 : fold_norm ? 5 : 7) + 2;
+    if (const char* dbg = std::getenv("B200_DEBUG_TX_LAUNCHES")) {   // debug: stop after k launches (tests/test_tx_layers_gpu.py)
+        const int k = std::atoi(dbg);
+        if (k >= 0 && k < plan->n_launches) plan->stop_after = k;
+    }
     return plan;
 }
 
 void TxPlan::run(cudaStream_t stream, ProfileSink* prof) {
-    nvtxRangePushA("Conv");
+    if (stop_after == 0) return;
+    // done(name) after every launch: marks it for the profile and says whether B200_DEBUG_TX_LAUNCHES stops the plan there
+    int launched = 0;
+    auto done = [&](const char* name) {
+        if (prof) prof->mark(name, stream);
+        if (++launched != stop_after) return false;
+        B200_CUDA(cudaGetLastError());
+        return true;
+    };
     {
+        NvtxRange r("Conv");
         const long long total = (long long)conv1.N * conv1.T * (conv1.C1 / 8);
         tx_conv1_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(conv1);
-        if (prof) prof->mark("tx_conv1", stream);
+        if (done("tx_conv1")) return;
+        for (auto& c : convs) {
+            run_gemm(c, stream);
+            if (done("tx_conv_gemm")) return;
+        }
     }
-    for (auto& c : convs) {
-        run_gemm(c, stream);
-        if (prof) prof->mark("tx_conv_gemm", stream);
-    }
-    nvtxRangePop();
     const unsigned norm_grid = (unsigned)((rows + 7) / 8);
-    nvtxRangePushA("TransEnc");
-    for (auto& L : layers) {
-        NvtxRange layer("TxLayerKoiTiled");
-        {
-            NvtxRange r("QKV+ROTE");
-            run_gemm(L.qkv, stream);
-            if (prof) prof->mark("qkv_gemm", stream);
-        }
-        {
-            NvtxRange r("MEA");
-            launch_attention(qkv_map, attn_tc_p, stream);
-            if (prof) prof->mark("tx_attention", stream);
-        }
-        {
-            NvtxRange r("OUTP");
-            run_gemm(L.out_proj, stream);
-            if (prof) prof->mark("out_proj_gemm", stream);
-        }
-        if (fp8) {
-            NvtxRange r("LNORM1");
-            rmsnorm_kernel<<<norm_grid, 256, 0, stream>>>(y, norm_out, L.n1, rows, norm_dim, norm_out8);
-            if (prof) prof->mark("rmsnorm_e4m3", stream);
-        } else if (!fold_norm) {
-            NvtxRange r("LNORM1");
-            rmsnorm_kernel<<<norm_grid, 256, 0, stream>>>(y, x, L.n1, rows, norm_dim, nullptr);
-            if (prof) prof->mark("rmsnorm", stream);
-        }
-        {
-            NvtxRange r("FC1+SILU");
-            run_gemm(L.fc1, stream);
-            if (prof) prof->mark("fc1_swiglu_gemm", stream);
-        }
-        {
-            NvtxRange r("FC2");
-            run_gemm(L.fc2, stream);
-            if (prof) prof->mark("fc2_gemm", stream);
-        }
-        if (!fold_norm) {
-            NvtxRange r("LNORM2");
-            rmsnorm_kernel<<<norm_grid, 256, 0, stream>>>(y, x, L.n2, rows, norm_dim, nullptr);
-            if (prof) prof->mark("rmsnorm", stream);
+    {
+        NvtxRange enc("TransEnc");
+        for (auto& L : layers) {
+            NvtxRange layer("TxLayerKoiTiled");
+            {
+                NvtxRange r("QKV+ROTE");
+                run_gemm(L.qkv, stream);
+                if (done("qkv_gemm")) return;
+            }
+            {
+                NvtxRange r("MEA");
+                launch_attention(qkv_map, attn_tc_p, stream);
+                if (done("tx_attention")) return;
+            }
+            {
+                NvtxRange r("OUTP");
+                run_gemm(L.out_proj, stream);
+                if (done("out_proj_gemm")) return;
+            }
+            if (fp8) {
+                NvtxRange r("LNORM1");
+                rmsnorm_kernel<<<norm_grid, 256, 0, stream>>>(y, norm_out, L.n1, rows, norm_dim, norm_out8);
+                if (done("rmsnorm_e4m3")) return;
+            } else if (!fold_norm) {
+                NvtxRange r("LNORM1");
+                rmsnorm_kernel<<<norm_grid, 256, 0, stream>>>(y, x, L.n1, rows, norm_dim, nullptr);
+                if (done("rmsnorm")) return;
+            }
+            {
+                NvtxRange r("FC1+SILU");
+                run_gemm(L.fc1, stream);
+                if (done("fc1_swiglu_gemm")) return;
+            }
+            {
+                NvtxRange r("FC2");
+                run_gemm(L.fc2, stream);
+                if (done("fc2_gemm")) return;
+            }
+            if (!fold_norm) {
+                NvtxRange r("LNORM2");
+                rmsnorm_kernel<<<norm_grid, 256, 0, stream>>>(y, x, L.n2, rows, norm_dim, nullptr);
+                if (done("rmsnorm")) return;
+            }
         }
     }
-    nvtxRangePop();
     {
         NvtxRange r("TransDec");
         run_gemm(upsample, stream);
-        if (prof) prof->mark("upsample_gemm", stream);
+        if (done("upsample_gemm")) return;
     }
     {
         NvtxRange r("CRF");
         run_gemm(crf, stream);
-        if (prof) prof->mark("crf_gemm", stream);
+        done("crf_gemm");
     }
     B200_CUDA(cudaGetLastError());
 }

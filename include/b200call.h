@@ -424,7 +424,19 @@ B200_API int b200_runner_profile(b200_runner* runner, int32_t num_chunks, char* 
  * "lstm_layer.ctas=32;lstm_layer.groups=2;lstm_layer.chunks_per_group=8".  Empty when every kernel spans the GPU. */
 B200_API int b200_runner_plan_info(const b200_runner* runner, char* buf, uint64_t buf_len);
 
-/* Debug: copy `bytes` of the runner's forward workspace (device) starting at `offset` to `dst` (host). */
+/* Debug: copy `bytes` of the runner's forward workspace (device) starting at `offset` to `dst` (host).
+ *
+ * Transformer models: the workspace holds, in this order and each block starting on a 256-byte boundary,
+ *   cbuf[0 .. num_convs - 2]   conv i's output, fp16 [N][t_i + 2 p_i + 16][size_i] with p_i = winlen_{i+1} / 2 zero rows
+ *                              in front (conv i + 1 reads them as its padding), t_i the time length after conv i
+ *   x, y, att                  fp16 [N * T][d_model] (T tokens per chunk)
+ *   qkv                        fp16 [N * T][3 * d_model]
+ *   hid                        fp16 [N * T][dim_feedforward]
+ *   ups                        fp16 [N * T][upsample_scale * d_model]
+ *   ss_a, ss_b                 fp32 [N * T][d_model / 32], partial sums of squares of the rows of x and of y
+ * B200_DEBUG_TX_LAUNCHES=k, set before the runner is created, makes its forwards return after the first k kernel
+ * launches of the plan (in the order b200_runner_profile lists them), so the buffers above can be read between any two
+ * launches.  Unset, or k at least the plan's launch count, runs the whole plan. */
 B200_API int b200_runner_debug_read_workspace(b200_runner* runner, uint64_t offset, uint64_t bytes, void* dst);
 
 /* ---- Modified-base models (conv_lstm_v3) -----------------------------------------------------------------------
