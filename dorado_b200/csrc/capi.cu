@@ -429,6 +429,23 @@ int b200_test_gemm_s8(int32_t device, const int8_t* a, const int8_t* b, const fl
     });
 }
 
+int b200_test_gemm_s8_scaled(int32_t device, const int8_t* a, const int8_t* b, const float* row_scale, const float* col_scale,
+                             int32_t M, int32_t N, int32_t K, int32_t activation, float theta, int32_t max_seq_len,
+                             int32_t rope_T, int32_t rope_cols, uint16_t* c) {
+    return guarded([&] {
+        if (!a || !b || !row_scale || !col_scale || !c) throw std::invalid_argument("b200_test_gemm_s8_scaled: null argument");
+        b200::test_gemm_s8_scaled_host(device, a, b, row_scale, col_scale, M, N, K, activation, theta, max_seq_len, rope_T,
+                                       rope_cols, c);
+    });
+}
+
+int b200_test_quantize_act_rows(int32_t device, const uint16_t* f16, int32_t rows, int32_t cols, int8_t* q, float* inv) {
+    return guarded([&] {
+        if (!f16 || !q || !inv) throw std::invalid_argument("b200_test_quantize_act_rows: null argument");
+        b200::test_quantize_act_rows_host(device, f16, rows, cols, q, inv);
+    });
+}
+
 int b200_test_quantize_rows(const uint16_t* f16, int32_t rows, int32_t cols, int8_t* q, uint16_t* scale) {
     return guarded([&] {
         if (rows < 1 || cols < 1 || !f16 || !q || !scale) throw std::invalid_argument("b200_test_quantize_rows: bad argument");

@@ -85,11 +85,12 @@ Engine::Engine(const b200_model_desc& desc, const b200_tensor* tensors, int num_
     if (desc.outsize != (1 << (2 * (desc.state_len + 1)))) throw std::invalid_argument("outsize != 4^(state_len+1)");
     if (desc.num_convs < 1 || desc.num_convs > 8) throw std::invalid_argument("num_convs must be in [1, 8]");
     if (desc.stride < 1) throw std::invalid_argument("stride must be positive");
-    if (desc.tx_precision != B200_TX_FP16 && desc.tx_precision != B200_TX_FP8_FFN) {
-        throw std::invalid_argument("tx_precision must be B200_TX_FP16 (0) or B200_TX_FP8_FFN (1)");
+    if (desc.tx_precision != B200_TX_FP16 && desc.tx_precision != B200_TX_FP8_FFN && desc.tx_precision != B200_TX_I8_QKV_FP8_FFN) {
+        throw std::invalid_argument("tx_precision must be B200_TX_FP16 (0), B200_TX_FP8_FFN (1) or B200_TX_I8_QKV_FP8_FFN (2)");
     }
-    if (desc.tx_precision == B200_TX_FP8_FFN && desc.model_type != B200_MODEL_TX) {
-        throw std::invalid_argument("the fp8_ffn precision applies to transformer models only; LSTM models run in fp16");
+    if (desc.tx_precision != B200_TX_FP16 && desc.model_type != B200_MODEL_TX) {
+        throw std::invalid_argument(std::string("the ") + (desc.tx_precision == B200_TX_FP8_FFN ? "fp8_ffn" : "int8_qkv_fp8_ffn") +
+                                    " precision applies to transformer models only; LSTM models run in fp16");
     }
     if (desc.lstm_precision != B200_LSTM_FP16 && desc.lstm_precision != B200_LSTM_INT8) {
         throw std::invalid_argument("lstm_precision must be B200_LSTM_FP16 (0) or B200_LSTM_INT8 (1)");

@@ -383,6 +383,12 @@ void test_gemm_fp8_host(int device, const uint8_t* a, const uint8_t* b, int M, i
 
 void test_gemm_s8_host(int device, const int8_t* a, const int8_t* b, const float* col_scale, const float* bias, int M, int N,
                        int K, int activation, uint16_t* c);
+void test_gemm_s8_scaled_host(int device, const int8_t* a, const int8_t* b, const float* row_scale, const float* col_scale,
+                              int M, int N, int K, int activation, float theta, int max_seq_len, int rope_T, int rope_cols,
+                              uint16_t* c);
+// The int8_qkv_fp8_ffn transformer's device quantiser (tx_model.cu) on host fp16 rows [rows][cols] (cols a multiple of
+// 128): int8 rows and the fp32 factor 1 / float(scale16) of each, bit for bit quantize_rows_f16's values
+void test_quantize_act_rows_host(int device, const uint16_t* f16, int rows, int cols, int8_t* q, float* inv);
 // Host quantisation of the int8_lstm weights (lstm_model.cu): utils::quantize_tensor(w, 1) on fp16 bits [rows][cols] ->
 // int8 and the fp16 scale of every row; and the fp32 factor 1 / (kInt8ActScale * scale) a row's accumulator is multiplied by
 void quantize_rows_f16(const uint16_t* w16, int rows, int cols, int8_t* q, uint16_t* scale16);

@@ -12,7 +12,8 @@
 // 128 E4M3 per 128-byte K row instead of 64 fp16, wgmma m64n32k32.e4m3 and the SwiGLU output cast to E4M3.
 // int8 form (template Q8 = GEMM_Q8_OPERANDS, the x-projection and the CRF linear of LSTM models in the int8_lstm precision):
 // the E4M3 form's ring and boxes, wgmma m64n32k32.s8 into s32 accumulators, which the epilogue converts and multiplies by a
-// per-column fp32 factor.  Q8 = GEMM_Q8_STORE is the fp16 form whose tanh epilogue stores int8 (those models' last conv).
+// per-column fp32 factor (and a per-row one with row_scale: the transformer's QKV + RoPE projection in the int8_qkv_fp8_ffn
+// precision).  Q8 = GEMM_Q8_STORE is the fp16 form whose tanh epilogue stores int8 (those models' last conv).
 // A is addressed through a 3-D tensor map (k, row, batch) so that overlapping-row views work: the last conv of the LSTM
 // models reads its im2col rows straight from the NTC activation buffer with row stride = stride * C_in (the reference's
 // "cutlass_conv" trick, ConvStack.cpp:236-275).
@@ -39,6 +40,9 @@ constexpr int BN_MAX = 128;
 constexpr int STAGES = 5;          // TMA -> wgmma ring depth: 5 x 32 KB of the 227 KB
 constexpr int GEMM_PARTS = 4;      // RMSNorm partial sums per row and column tile (GemmDesc::out_ss): one per 32-column chunk
 constexpr int GEMM_THREADS = 384;  // warpgroup 0: producer; warpgroups 1, 2: MMA + epilogue of 64 rows each
+// Kernel form (template Q8) of GEMM_Q8_OPERANDS with GemmDesc::row_scale: its own instantiations, so that the int8 forms
+// without row factors keep their code
+constexpr int Q8_OPERANDS_ROWS = 3;
 
 struct GemmKernelParams {
     int rows_per_batch, tiles_per_batch, N, num_k_blocks, bn;
@@ -60,6 +64,7 @@ struct GemmKernelParams {
     int a_ss_parts, res_ss_parts;
     float norm_inv_dim, norm_eps;
     const float* col_scale;   // GEMM_Q8_OPERANDS
+    const float* row_scale;   // GEMM_Q8_OPERANDS, optional
 };
 
 // i-th tile of this CTA: row tile mt, column tile nt; false when the CTA has run out of tiles.  Producer and consumers walk
@@ -111,7 +116,8 @@ template <int ACT, bool FP8, int Q8 = GEMM_Q8_NONE>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a,
                                                                      const __grid_constant__ CUtensorMap tma_w,
                                                                      const GemmKernelParams p) {
-    constexpr bool S8 = Q8 == GEMM_Q8_OPERANDS;
+    constexpr bool ROWS = Q8 == Q8_OPERANDS_ROWS;
+    constexpr bool S8 = Q8 == GEMM_Q8_OPERANDS || ROWS;
     constexpr int KB = FP8 || S8 ? BK8 : BK;   // K elements per block
     using Acc = std::conditional_t<S8, int32_t, float>;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -205,6 +211,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
         bool valid[2];
         long long g[2], off[2];
         float r_a[2], r_res[2];
+        float r_q[2];   // int8 operands with row factors: the A row's dequantisation factor (GemmDesc::row_scale)
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int row = r0 + rloc + 8 * h;
@@ -212,6 +219,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
             const uint32_t g32 = (uint32_t)(batch * p.rows_per_batch + row);
             g[h] = g32;
             off[h] = valid[h] ? (long long)(g32 / p.out_m1) * p.out_s0 + (long long)(g32 % p.out_m1) * p.out_s1 : 0;
+            if constexpr (ROWS) {
+                r_q[h] = valid[h] ? __ldg(p.row_scale + g[h]) : 0.0f;
+            }
             // folded RMSNorm: 1/rms of this row of A and of the residual row, from the partial sums of squares (fixed order)
             r_a[h] = 1.0f;
             r_res[h] = 1.0f;
@@ -226,8 +236,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                 r_res[h] = rsqrtf(ss * p.norm_inv_dim + p.norm_eps);
             }
         }
-        if constexpr (S8) {
-            // s32 -> fp32 is exact for the K this form is used at (|acc| <= 127^2 K < 2^24 up to K = 1024)
+        if constexpr (S8 && ACT != GEMM_ACT_ROPE) {
+            // s32 -> fp32 (cvt.rn) is exact up to |acc| = 2^24 (127^2 K < 2^24 up to K = 1024); beyond it rounds to nearest
+            // even.  With row factors: v = (float(acc) * row) * col (+ bias), the second product fused with the bias.
 #pragma unroll
             for (int c = 0; c < BN_MAX / 32; ++c) {
                 if (c >= nch) continue;
@@ -240,8 +251,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         if (!valid[h]) continue;
-                        const float v0 = fmaf((float)acc[c][4 * j + 2 * h], sc.x, b2.x);
-                        const float v1 = fmaf((float)acc[c][4 * j + 2 * h + 1], sc.y, b2.y);
+                        float v0, v1;
+                        if constexpr (ROWS) {
+                            v0 = fmaf(__fmul_rn((float)acc[c][4 * j + 2 * h], r_q[h]), sc.x, b2.x);
+                            v1 = fmaf(__fmul_rn((float)acc[c][4 * j + 2 * h + 1], r_q[h]), sc.y, b2.y);
+                        } else {
+                            v0 = fmaf((float)acc[c][4 * j + 2 * h], sc.x, b2.x);
+                            v1 = fmaf((float)acc[c][4 * j + 2 * h + 1], sc.y, b2.y);
+                        }
                         *reinterpret_cast<__half2*>(p.out + off[h] + nc) = __floats2half2_rn(act_apply<ACT>(v0), act_apply<ACT>(v1));
                     }
                 }
@@ -260,8 +277,21 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
 #pragma unroll
                         for (int j = 0; j < 4; ++j) {
                             const int col = 8 * j + 2 * quad;   // column pair (col, col + 1) of x1; x2 is 32 columns on
-                            float a0 = acc[c][4 * j + 2 * h] * r_a[h], a1 = acc[c][4 * j + 2 * h + 1] * r_a[h];
-                            float b0 = acc[c + 1][4 * j + 2 * h] * r_a[h], b1 = acc[c + 1][4 * j + 2 * h + 1] * r_a[h];
+                            float a0, a1, b0, b1;
+                            if constexpr (S8) {
+                                // (float(acc) * row factor) * column factor, in that order
+                                const float2 ca = __ldg(reinterpret_cast<const float2*>(p.col_scale + nc0 + col));
+                                const float2 cb = __ldg(reinterpret_cast<const float2*>(p.col_scale + nc0 + 32 + col));
+                                a0 = __fmul_rn(__fmul_rn(__int2float_rn(acc[c][4 * j + 2 * h]), r_q[h]), ca.x);
+                                a1 = __fmul_rn(__fmul_rn(__int2float_rn(acc[c][4 * j + 2 * h + 1]), r_q[h]), ca.y);
+                                b0 = __fmul_rn(__fmul_rn(__int2float_rn(acc[c + 1][4 * j + 2 * h]), r_q[h]), cb.x);
+                                b1 = __fmul_rn(__fmul_rn(__int2float_rn(acc[c + 1][4 * j + 2 * h + 1]), r_q[h]), cb.y);
+                            } else {
+                                a0 = acc[c][4 * j + 2 * h] * r_a[h];
+                                a1 = acc[c][4 * j + 2 * h + 1] * r_a[h];
+                                b0 = acc[c + 1][4 * j + 2 * h] * r_a[h];
+                                b1 = acc[c + 1][4 * j + 2 * h + 1] * r_a[h];
+                            }
                             if (rot) {
                                 const float4 cs = __ldg(tab + (size_t)(col / 2) * p.rope_stride);
                                 const float x0 = cs.x * a0 - cs.y * b0, y0 = cs.y * a0 + cs.x * b0;
@@ -419,14 +449,19 @@ GemmPlan make_gemm_plan(const GemmDesc& d) {
     }
     if (d.q8 != GEMM_Q8_NONE) {
         const bool plain = !d.fp8 && !d.residual && !d.out_ss && !d.a_ss && !d.res_ss;
-        if (s8 && !(plain && d.col_scale && (d.act == GEMM_ACT_NONE || d.act == GEMM_ACT_TANH_X5))) {
+        if (s8 && !d.row_scale && !(plain && d.col_scale && (d.act == GEMM_ACT_NONE || d.act == GEMM_ACT_TANH_X5))) {
             throw std::invalid_argument("gemm: int8 operands take col_scale, a column bias and the plain or TANH_X5 epilogue only");
+        }
+        if (s8 && d.row_scale && !(plain && d.col_scale && (d.act == GEMM_ACT_NONE || (d.act == GEMM_ACT_ROPE && !d.bias)))) {
+            throw std::invalid_argument("gemm: int8 operands with row_scale take col_scale and the plain (with a column bias) or "
+                                        "the RoPE epilogue (without) only");
         }
         if (d.q8 == GEMM_Q8_STORE && !(plain && d.act == GEMM_ACT_TANH)) {
             throw std::invalid_argument("gemm: the int8 store goes with fp16 operands and the TANH epilogue only");
         }
         if (!s8 && d.q8 != GEMM_Q8_STORE) throw std::invalid_argument("gemm: unknown q8 form");
     }
+    if (d.row_scale && !s8) throw std::invalid_argument("gemm: row_scale goes with int8 operands only");
     if (d.fp8 && (d.act != GEMM_ACT_NONE && d.act != GEMM_ACT_SWIGLU)) {
         throw std::invalid_argument("gemm: E4M3 operands take the plain and SwiGLU epilogues only");
     }
@@ -509,6 +544,7 @@ void run_gemm(const GemmPlan& p, cudaStream_t stream) {
     k.norm_inv_dim = p.d.norm_dim > 0 ? 1.0f / (float)p.d.norm_dim : 0.0f;
     k.norm_eps = p.d.norm_eps;
     k.col_scale = p.d.col_scale;
+    k.row_scale = p.d.row_scale;
     const int max_ctas = p.d.max_ctas > 0 && p.d.max_ctas < kNumSMs ? p.d.max_ctas : kNumSMs;
     const int grid = k.num_tiles < max_ctas ? k.num_tiles : max_ctas;
     if (p.d.fp8) {
@@ -520,6 +556,8 @@ void run_gemm(const GemmPlan& p, cudaStream_t stream) {
     if (p.d.q8 != GEMM_Q8_NONE) {
         if (p.d.q8 == GEMM_Q8_STORE) launch_gemm<GEMM_ACT_TANH, false, GEMM_Q8_STORE>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
         else if (p.d.act == GEMM_ACT_TANH_X5) launch_gemm<GEMM_ACT_TANH_X5, false, GEMM_Q8_OPERANDS>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
+        else if (p.d.act == GEMM_ACT_ROPE) launch_gemm<GEMM_ACT_ROPE, false, Q8_OPERANDS_ROWS>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
+        else if (p.d.row_scale) launch_gemm<GEMM_ACT_NONE, false, Q8_OPERANDS_ROWS>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
         else launch_gemm<GEMM_ACT_NONE, false, GEMM_Q8_OPERANDS>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
         B200_CUDA(cudaGetLastError());
         return;
@@ -744,32 +782,40 @@ void test_gemm_fp8_host(int device, const uint8_t* a, const uint8_t* b, int M, i
     B200_CUDA(cudaMemcpy(c, d_c, out_bytes, cudaMemcpyDeviceToHost));
 }
 
-// int8 operands (A [M][K], W [N][K], K zero-padded to a multiple of 128): c = act(float(A W^T) * col_scale[n] + bias[n]), fp16
-void test_gemm_s8_host(int device, const int8_t* a, const int8_t* b, const float* col_scale, const float* bias, int M, int N,
-                       int K, int activation, uint16_t* c) {
-    if (M < 1 || N < 1 || K < 1) throw std::invalid_argument("test_gemm_s8: empty operand");
+namespace {
+
+// The int8 GEMM on host operands (A [M][K], W [N][K], K zero-padded to a multiple of 128 here) into fp16 c [M][N]: the
+// descriptor's factors, bias and RoPE table (rope: empty, or rope_table()'s positions per dim pair) as given
+void gemm_s8_host(int device, const int8_t* a, const int8_t* b, const float* row_scale, const float* col_scale,
+                  const float* bias, int M, int N, int K, int activation, const std::vector<float>& rope, int max_seq_len,
+                  int rope_T, int rope_cols, uint16_t* c) {
     require_sm90(device);
     const int Kp = (K + BK8 - 1) / BK8 * BK8;
     int8_t *d_a = nullptr, *d_w = nullptr;
-    float *d_scale = nullptr, *d_bias = nullptr;
+    float *d_row = nullptr, *d_scale = nullptr, *d_bias = nullptr, *d_rope = nullptr;
     __half* d_c = nullptr;
     Arena arena;
     arena.allocate([&](Bump& bump) {
         d_a = bump.take<int8_t>((size_t)M * Kp);
         d_w = bump.take<int8_t>((size_t)N * Kp);
+        d_row = bump.take<float>((size_t)M * 4);
         d_scale = bump.take<float>((size_t)N * 4);
         d_bias = bump.take<float>((size_t)N * 4);
+        d_rope = bump.take<float>((rope.empty() ? 1 : rope.size()) * 4);
         d_c = bump.take<__half>((size_t)M * N * 2);
     });
     B200_CUDA(cudaMemset(d_a, 0, (size_t)M * Kp));
     B200_CUDA(cudaMemset(d_w, 0, (size_t)N * Kp));
     B200_CUDA(cudaMemcpy2D(d_a, (size_t)Kp, a, (size_t)K, (size_t)K, M, cudaMemcpyHostToDevice));
     B200_CUDA(cudaMemcpy2D(d_w, (size_t)Kp, b, (size_t)K, (size_t)K, N, cudaMemcpyHostToDevice));
+    if (row_scale) B200_CUDA(cudaMemcpy(d_row, row_scale, (size_t)M * 4, cudaMemcpyHostToDevice));
     B200_CUDA(cudaMemcpy(d_scale, col_scale, (size_t)N * 4, cudaMemcpyHostToDevice));
     if (bias) B200_CUDA(cudaMemcpy(d_bias, bias, (size_t)N * 4, cudaMemcpyHostToDevice));
+    if (!rope.empty()) B200_CUDA(cudaMemcpy(d_rope, rope.data(), rope.size() * 4, cudaMemcpyHostToDevice));
     GemmDesc d{};
     d.q8 = GEMM_Q8_OPERANDS;
     d.col_scale = d_scale;
+    d.row_scale = row_scale ? d_row : nullptr;
     d.a = d_a;
     d.batches = 1;
     d.rows_per_batch = M;
@@ -784,10 +830,42 @@ void test_gemm_s8_host(int device, const int8_t* a, const int8_t* b, const float
     d.out_m1 = 1;
     d.out_s0 = N;
     d.out_s1 = 0;
+    if (!rope.empty()) {
+        d.rope = d_rope;
+        d.rope_T = rope_T;
+        d.rope_cols = rope_cols;
+        d.rope_stride = max_seq_len;
+    }
     const GemmPlan plan = make_gemm_plan(d);
     run_gemm(plan, nullptr);
     B200_CUDA(cudaDeviceSynchronize());
     B200_CUDA(cudaMemcpy(c, d_c, (size_t)M * N * 2, cudaMemcpyDeviceToHost));
+}
+
+}  // namespace
+
+// int8 operands (A [M][K], W [N][K], K zero-padded to a multiple of 128): c = act(float(A W^T) * col_scale[n] + bias[n]), fp16
+void test_gemm_s8_host(int device, const int8_t* a, const int8_t* b, const float* col_scale, const float* bias, int M, int N,
+                       int K, int activation, uint16_t* c) {
+    if (M < 1 || N < 1 || K < 1) throw std::invalid_argument("test_gemm_s8: empty operand");
+    gemm_s8_host(device, a, b, nullptr, col_scale, bias, M, N, K, activation, {}, 0, 0, 0, c);
+}
+
+// int8 operands with per-row and per-column factors: v = (float(A W^T) * row_scale[m]) * col_scale[n]; c = fp16(v), or with
+// GEMM_ACT_ROPE the rotary embedding of v at position m % rope_T on the first rope_cols columns (the table of
+// rope_table(theta, max_seq_len)), as the transformer's QKV projection.
+void test_gemm_s8_scaled_host(int device, const int8_t* a, const int8_t* b, const float* row_scale, const float* col_scale,
+                              int M, int N, int K, int activation, float theta, int max_seq_len, int rope_T, int rope_cols,
+                              uint16_t* c) {
+    if (M < 1 || N < 1 || K < 1 || N % 32 != 0) throw std::invalid_argument("test_gemm_s8_scaled: empty operand or N not a multiple of 32");
+    if (activation != GEMM_ACT_NONE && activation != GEMM_ACT_ROPE) throw std::invalid_argument("test_gemm_s8_scaled: plain or RoPE only");
+    const bool rope = activation == GEMM_ACT_ROPE;
+    if (rope && !(theta > 0.0f && max_seq_len >= 1 && max_seq_len <= (1 << 16) && rope_T >= 1 && rope_T <= max_seq_len &&
+                  rope_cols >= 0 && rope_cols <= N && rope_cols % 64 == 0 && N % 64 == 0)) {
+        throw std::invalid_argument("test_gemm_s8_scaled: RoPE needs theta > 0, 1 <= rope_T <= max_seq_len and whole 64-column heads");
+    }
+    gemm_s8_host(device, a, b, row_scale, col_scale, nullptr, M, N, K, activation,
+                 rope ? rope_table(theta, max_seq_len) : std::vector<float>(), max_seq_len, rope_T, rope_cols, c);
 }
 
 }  // namespace b200

@@ -21,6 +21,7 @@ enum GemmAct : int {
 enum GemmQ8 : int {
     GEMM_Q8_NONE = 0,
     GEMM_Q8_OPERANDS = 1,  // A and W are int8: exact s32 accumulation, out = act(float(acc) * col_scale[n] + bias[n]) as fp16
+                           // (float(acc) * row_scale[g] first when GemmDesc::row_scale is set)
     GEMM_Q8_STORE = 2,     // fp16 operands, GEMM_ACT_TANH: the output is int8 cvt.rni.sat(kInt8ActScale * tanh(v))
 };
 // int8 value of an activation v in [-1, 1] (the last convolution's tanh output and every h_t of an int8 LSTM layer).  The
@@ -34,8 +35,12 @@ struct GemmDesc {
     // q8: GemmQ8.  GEMM_Q8_OPERANDS takes int8 bytes with the E4M3 form's addressing (K a multiple of 128), the plain and
     // TANH_X5 activations, a column bias and col_scale [N] (fp32 dequantisation factor per output column).
     // GEMM_Q8_STORE writes int8 where the fp16 form writes fp16: out is int8 and its strides count bytes.
+    // row_scale [batches * rows_per_batch] (optional, GEMM_Q8_OPERANDS only): fp32 dequantisation factor per A row, applied
+    // as v = (float(acc) * row_scale[g]) * col_scale[n], each product rounded in fp32.  With it the form also takes
+    // GEMM_ACT_ROPE (no bias), whose rotation then runs on v (the int8_qkv_fp8_ffn transformer's QKV projection).
     int q8 = GEMM_Q8_NONE;
     const float* col_scale = nullptr;
+    const float* row_scale = nullptr;
     // A: logical [batches][rows_per_batch][K] fp16, K contiguous; row/batch strides in elements
     const void* a = nullptr;
     int batches = 1;

@@ -19,6 +19,12 @@
 // 596-697): fc1 and fc2 take E4M3 operands.  norm1 is an explicit pass that writes the fp16 row (fc2's residual) and its
 // E4M3 copy (fc1's A); fc1 + SwiGLU writes E4M3 (fc2's A); fc2 writes fp16.  The fp16 weights the reference keeps (QKV,
 // out_proj, both RMSNorm gains) lose their low 4 mantissa bits first (remove_bits, TxModules.cpp:104-111, 443-453).
+//
+// Precision B200_TX_I8_QKV_FP8_FFN (koi_use_f8 = 1 with koi_use_i8 = 1, the reference's default on an H100: TxModules.cpp:477-479,
+// 936-961, 497-506, 611-616, 669, 713): as fp8_ffn, but the fused QKV + RoPE projection takes int8 operands.  Wqkv is
+// quantised per output row from the fp16 weights before remove_bits; the stack's input is quantised per token row by a device
+// pass, and norm2 becomes an explicit pass that writes the next layer's fp16 rows and their int8 copy.  Nothing is folded:
+// out_proj's residual and the upsample read the normalised fp16 rows.
 #include "engine.h"
 #include "gemm.h"
 #include "nvtx.h"
@@ -97,14 +103,69 @@ __global__ void __launch_bounds__(256) tx_conv1_kernel(const Conv1Params p) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// Per-row int8 quantisation of fp16 rows (the QKV projection's A in the int8_qkv_fp8_ffn precision), by the warp of a row
+// whose lane holds `per` consecutive columns from src (absmax: the largest |x| of the lane's columns): utils::quantize_tensor
+// (tensor_utils.cpp:293-300) as torch evaluates it on fp16, i.e. quantize_rows_f16's arithmetic --
+//     scale16 = fp16(128 / absmax)   q = clip(rne(fp16(x * scale16)), -127, 127)   inv = 1 / float(scale16)
+// with the reference's reciprocal of the scale (TxModules.cpp:958).  An all-zero row gets q = 0; a row whose scale overflows
+// to +inf (absmax 0, or below about 128 / 65520) gets inv = 0, and there a zero element's product 0 * inf is NaN, which the
+// clip takes to -127 as quantize_rows_f16 does (fmaxf, std::max): q is defined everywhere and such rows contribute 0.
+__device__ __forceinline__ void quantize_row_i8(const __half* src, int per, float absmax, int lane, int8_t* q, float* inv) {
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) absmax = fmaxf(absmax, __shfl_xor_sync(0xffffffffu, absmax, o));
+    const float scale = __half2float(__float2half_rn(__fdiv_rn(128.0f, absmax)));
+    if (lane == 0) *inv = __fdiv_rn(1.0f, scale);
+    for (int i = 0; i < per; i += 4) {
+        const uint2 v = *reinterpret_cast<const uint2*>(src + i);
+        const __half* h = reinterpret_cast<const __half*>(&v);
+        uint32_t packed = 0;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            int qv = 0;
+            if (absmax != 0.0f) {
+                const float prod = __half2float(__float2half_rn(__fmul_rn(__half2float(h[e]), scale)));
+                qv = (int)fminf(127.0f, fmaxf(-127.0f, rintf(prod)));
+            }
+            packed |= (uint32_t)(qv & 0xff) << (8 * e);
+        }
+        *reinterpret_cast<uint32_t*>(q + i) = packed;
+    }
+}
+
+// The stack input's int8 copy (int8_qkv_fp8_ffn): quantize_row_i8 of every fp16 row of in [rows][dim], one warp per row
+__global__ void __launch_bounds__(256) quantize_i8_kernel(const __half* __restrict__ in, long long rows, int dim,
+                                                          int8_t* __restrict__ q, float* __restrict__ inv) {
+    const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (row >= rows) return;
+    const int per = dim / 32;
+    const __half* src = in + row * dim + lane * per;
+    float absmax = 0.0f;
+    for (int i = 0; i < per; i += 4) {
+        const uint2 v = *reinterpret_cast<const uint2*>(src + i);
+        const __half2* h = reinterpret_cast<const __half2*>(&v);
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+            const float2 a = __half22float2(h[j]);
+            absmax = fmaxf(absmax, fmaxf(fabsf(a.x), fabsf(a.y)));
+        }
+    }
+    quantize_row_i8(src, per, absmax, lane, q + row * dim + lane * per, inv + row);
+}
+
+// ------------------------------------------------------------------------------------------------
 // RMSNorm over rows of `dim` (RMSNorm.cpp:14-18): x * rsqrt(mean(x^2) + eps) * w ; one warp per row, lane i owns the dim / 32
 // consecutive columns from i * dim / 32 (dim a multiple of 128, so whole 8-byte groups).  The row is read twice (sum of
 // squares, then the scaled store) rather than held in registers, so one kernel serves every width.
 // ------------------------------------------------------------------------------------------------
 // out8 (optional): the E4M3 cast of the fp16 values written to out, same layout (fc1's A in the fp8_ffn precision).
+// outq / out_inv (optional): quantize_row_i8 of the fp16 values written to out (norm2 in the int8_qkv_fp8_ffn precision: the
+// next QKV projection's A).  Koi's requantisation inside koi_rmsnorm_residual is closed source; quantising the stored fp16
+// row with the stack input's arithmetic is this engine's choice.
 __global__ void __launch_bounds__(256) rmsnorm_kernel(const __half* __restrict__ in, __half* __restrict__ out,
                                                       const float* __restrict__ w, long long rows, int dim,
-                                                      uint8_t* __restrict__ out8) {
+                                                      uint8_t* __restrict__ out8, int8_t* __restrict__ outq,
+                                                      float* __restrict__ out_inv) {
     const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (row >= rows) return;
@@ -124,6 +185,7 @@ __global__ void __launch_bounds__(256) rmsnorm_kernel(const __half* __restrict__
     for (int o = 16; o >= 1; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
     const float rstd = rsqrtf(ss * (1.0f / (float)dim) + 1e-5f);
     __half* dst = out + row * dim + lane * per;
+    float absmax = 0.0f;   // of the fp16 values stored (outq)
     for (int i = 0; i < per; i += 4) {
         const uint2 v = *reinterpret_cast<const uint2*>(src + i);
         const __half2* h = reinterpret_cast<const __half2*>(&v);
@@ -135,12 +197,18 @@ __global__ void __launch_bounds__(256) rmsnorm_kernel(const __half* __restrict__
             o2[j] = __floats2half2_rn(a.x * rstd * __ldg(w + c), a.y * rstd * __ldg(w + c + 1));
         }
         *reinterpret_cast<uint2*>(dst + i) = *reinterpret_cast<uint2*>(o2);
+        if (outq) {
+            const float2 f0 = __half22float2(o2[0]), f1 = __half22float2(o2[1]);
+            absmax = fmaxf(absmax, fmaxf(fmaxf(fabsf(f0.x), fabsf(f0.y)), fmaxf(fabsf(f1.x), fabsf(f1.y))));
+        }
         if (out8) {
             const float2 f0 = __half22float2(o2[0]), f1 = __half22float2(o2[1]);
             const uint32_t q = (uint32_t)tc::cvt_e4m3x2(f0.x, f0.y) | ((uint32_t)tc::cvt_e4m3x2(f1.x, f1.y) << 16);
             *reinterpret_cast<uint32_t*>(out8 + row * dim + lane * per + i) = q;
         }
     }
+    // the lane reads back its own stores
+    if (outq) quantize_row_i8(dst, per, absmax, lane, outq + row * dim + lane * per, out_inv + row);
 }
 
 constexpr int ATT_D = 64;   // head dimension
@@ -369,6 +437,8 @@ void launch_attention(const CUtensorMap& qkv_map, const AttnTcParams& p, cudaStr
 struct TxLayerWeights {
     __half *wqkv = nullptr, *wo = nullptr, *w1 = nullptr, *w2 = nullptr;
     uint8_t *w1_e4m3 = nullptr, *w2_e4m3 = nullptr;   // fp8_ffn: fc1 (interleaved rows) and fc2 as E4M3 (w1, w2 unused)
+    int8_t* wqkv_i8 = nullptr;                         // int8_qkv_fp8_ffn: Wqkv per output row (wqkv unused)
+    float* wqkv_inv = nullptr;                         // and the fp32 factor 1 / float(scale16) of each row
     float *bo = nullptr, *n1 = nullptr, *n2 = nullptr;
 };
 
@@ -384,7 +454,7 @@ public:
         GemmPlan qkv, out_proj, fc1, fc2;
         const float *n1, *n2;
     };
-    std::string info() const override { return fp8 ? "tx.fp8_ffn=1" : std::string(); }
+    std::string info() const override { return i8 ? "tx.fp8_ffn=1;tx.int8_qkv=1" : fp8 ? "tx.fp8_ffn=1" : std::string(); }
     std::vector<Layer> layers;
     GemmPlan upsample, crf;
     CUtensorMap qkv_map;       // qkv as [N*T][3*H*64], box 64 x 128 (Q, K and V tiles of the tensor-core attention)
@@ -397,8 +467,11 @@ public:
     int stop_after = -1;        // B200_DEBUG_TX_LAUNCHES: run() returns after this many launches (-1: the whole plan)
     bool fold_norm = true;
     bool fp8 = false;           // fp8_ffn: explicit norm1 pass writing fp16 (norm_out) and E4M3 (norm_out8), E4M3 fc1 / fc2
+    bool i8 = false;            // int8_qkv_fp8_ffn (fp8 set too): stack input quantise pass, norm2 writing x8 / x_inv, int8 qkv
     __half* norm_out = nullptr;
     uint8_t* norm_out8 = nullptr;
+    int8_t* x8 = nullptr;       // int8 copy of x's rows and their factors (int8_qkv_fp8_ffn)
+    float* x_inv = nullptr;
 };
 
 class TxModel final : public Model {
@@ -409,8 +482,11 @@ public:
     std::unique_ptr<ForwardPlan> make_plan(int N, int T_in, const __half* signal, __half* scores, void* ws,
                                            size_t ws_bytes) override;
     b200_model_desc desc;
-    bool fold_norm = true;   // B200_TX_RMSNORM_PASS=1: separate RMSNorm kernel after every sub-layer (A/B comparisons)
-    bool fp8 = false;        // desc.tx_precision == B200_TX_FP8_FFN (norm2 stays folded; the RMSNorm-pass option is ignored)
+    // B200_TX_RMSNORM_PASS=1: separate RMSNorm kernel after every sub-layer (A/B comparisons).  false in int8_qkv_fp8_ffn,
+    // where both norms are explicit passes and no gain is folded into a weight
+    bool fold_norm = true;
+    bool fp8 = false;        // B200_TX_FP8_FFN or B200_TX_I8_QKV_FP8_FFN (fp8_ffn: norm2 stays folded; the RMSNorm-pass option is ignored)
+    bool i8 = false;         // B200_TX_I8_QKV_FP8_FFN
     float* conv1_w = nullptr;
     std::vector<__half*> conv_w;  // conv 2..n  [C_out][W*C_in]
     std::vector<float*> conv_b;
@@ -431,6 +507,8 @@ private:
         std::vector<__half*> cbuf;  // output of conv i (but the last), [N][t_pad[i]][size]
         __half *x, *y, *att, *qkv, *hid, *ups;
         float *ss_a, *ss_b;  // partial sums of squares (folded RMSNorm) of the rows in x and in y
+        int8_t* x8;          // int8_qkv_fp8_ffn: the int8 copy of x's rows [rows][d_model] and their factors [rows]
+        float* x_inv;        // (both null in the other precisions)
     };
     // The workspace layout for N chunks of T_in samples; refuses a chunk longer than the RoPE table
     Buffers carve(Bump& b, int N, int T_in) const;
@@ -451,8 +529,10 @@ TxModel::Shapes TxModel::shapes(int T_in) const {
 }
 
 TxModel::TxModel(const b200_model_desc& d, const b200_tensor* tensors, int n) : desc(d) {
-    fp8 = d.tx_precision == B200_TX_FP8_FFN;
+    i8 = d.tx_precision == B200_TX_I8_QKV_FP8_FFN;
+    fp8 = d.tx_precision == B200_TX_FP8_FFN || i8;
     if (const char* e = std::getenv("B200_TX_RMSNORM_PASS"); e && !fp8) fold_norm = std::atoi(e) == 0;
+    if (i8) fold_norm = false;
     // the shapes the kernels handle: head dimension 64 (attention, RoPE epilogue), d_model in whole 128-column tiles (the
     // folded RMSNorm's partial sums), K of the fc2 GEMM in whole 64-wide blocks, key bands of at most AT_MAXBLK blocks
     if (d.nhead < 1 || d.d_model != ATT_D * d.nhead) throw Unsupported("transformer path needs d_model == 64 * nhead (head dimension 64)");
@@ -460,7 +540,8 @@ TxModel::TxModel(const b200_model_desc& d, const b200_tensor* tensors, int n) : 
     if (d.dim_feedforward < 64 || d.dim_feedforward % 64 != 0) throw Unsupported("transformer path needs dim_feedforward a multiple of 64");
     check_attention_window(d.attn_window_upper, d.attn_window_lower);
     if (fp8 && d.dim_feedforward % 128 != 0) {
-        throw Unsupported("fp8_ffn precision needs dim_feedforward a multiple of 128 (fc2's K in whole 128-byte E4M3 blocks)");
+        throw Unsupported(std::string(i8 ? "int8_qkv_fp8_ffn" : "fp8_ffn") +
+                          " precision needs dim_feedforward a multiple of 128 (fc2's K in whole 128-byte E4M3 blocks)");
     }
     if (d.num_convs < 2 || d.convs[0].insize != 1 || d.convs[0].stride != 1 || d.convs[0].winlen > 9 || d.convs[0].size % 8) {
         throw Unsupported("transformer conv stack shape not supported");
@@ -518,14 +599,17 @@ TxModel::TxModel(const b200_model_desc& d, const b200_tensor* tensors, int n) : 
         rounded.push_back(fp8 ? fp16_remove_bits(v, cnt, 4) : std::vector<float>(v, v + cnt));
         return rounded.back().data();
     };
-    auto up8 = [&](const float* v, size_t cnt) {
-        std::vector<uint8_t> q(cnt);
-        for (size_t i = 0; i < cnt; ++i) q[i] = e4m3_from_f16_bits(f16_bits(v[i]));
+    auto up_bytes = [&](const void* data, size_t cnt) {
         void* p = nullptr;
         B200_CUDA(cudaMalloc(&p, cnt));
         owned.push_back(p);
-        B200_CUDA(cudaMemcpy(p, q.data(), cnt, cudaMemcpyHostToDevice));
-        return static_cast<uint8_t*>(p);
+        B200_CUDA(cudaMemcpy(p, data, cnt, cudaMemcpyHostToDevice));
+        return p;
+    };
+    auto up8 = [&](const float* v, size_t cnt) {
+        std::vector<uint8_t> q(cnt);
+        for (size_t i = 0; i < cnt; ++i) q[i] = e4m3_from_f16_bits(f16_bits(v[i]));
+        return static_cast<uint8_t*>(up_bytes(q.data(), cnt));
     };
     for (int l = 0; l < d.depth; ++l) {
         const std::string pfx = "transformer_encoder." + std::to_string(l) + ".";
@@ -533,8 +617,28 @@ TxModel::TxModel(const b200_model_desc& d, const b200_tensor* tensors, int n) : 
         const float* n1 = rb(find_tensor(tensors, n, pfx + "norm1.weight.tensor").data, dm);
         const float* n2 = rb(find_tensor(tensors, n, pfx + "norm2.weight.tensor").data, dm);
         const auto& wqkv_t = find_tensor(tensors, n, pfx + "self_attn.Wqkv.weight.tensor");
-        const float* wqkv = rb(wqkv_t.data, (size_t)3 * dm * dm);
-        lw.wqkv = up16(fold_norm ? fold(wqkv, (size_t)3 * dm, prev_gain) : std::vector<float>(wqkv, wqkv + (size_t)3 * dm * dm));
+        if (i8) {
+            // quantize_tensor(fp16(Wqkv), -1), one scale per output row, from the fp16 weights as they are BEFORE remove_bits
+            // (the reference quantises at TxModules.cpp:499 and rounds at :589); its Q / K row interleave (:488-496) moves
+            // rows without changing any, so the engine's row order stays.  No gain in the columns: norm2 is a pass here.
+            const size_t cnt = (size_t)3 * dm * dm;
+            std::vector<uint16_t> h(cnt);
+            for (size_t i = 0; i < cnt; ++i) h[i] = f16_bits(wqkv_t.data[i]);
+            std::vector<int8_t> q(cnt);
+            std::vector<uint16_t> scale((size_t)3 * dm);
+            quantize_rows_f16(h.data(), 3 * dm, dm, q.data(), scale.data());
+            std::vector<float> inv((size_t)3 * dm);
+            for (int r = 0; r < 3 * dm; ++r) {
+                __half_raw raw;
+                raw.x = scale[r];
+                inv[r] = 1.0f / __half2float(__half(raw));   // scale.reciprocal_(): 0 for an infinite scale
+            }
+            lw.wqkv_i8 = reinterpret_cast<int8_t*>(up_bytes(q.data(), cnt));
+            lw.wqkv_inv = up32(inv.data(), inv.size());
+        } else {
+            const float* wqkv = rb(wqkv_t.data, (size_t)3 * dm * dm);
+            lw.wqkv = up16(fold_norm ? fold(wqkv, (size_t)3 * dm, prev_gain) : std::vector<float>(wqkv, wqkv + (size_t)3 * dm * dm));
+        }
         const float* wo = rb(find_tensor(tensors, n, pfx + "self_attn.out_proj.weight.tensor").data, (size_t)dm * dm);
         lw.wo = up16(std::vector<float>(wo, wo + (size_t)dm * dm));
         lw.bo = up32(find_tensor(tensors, n, pfx + "self_attn.out_proj.bias.tensor").data, dm);
@@ -598,6 +702,14 @@ TxModel::Buffers TxModel::carve(Bump& b, int N, int T_in) const {
     w.ups = b.take<__half>(rows * desc.upsample_scale * dm * 2);
     w.ss_a = b.take<float>(rows * gemm_out_ss_parts((int)dm) * 4);   // x: after fc2 / the previous layer
     w.ss_b = b.take<float>(rows * gemm_out_ss_parts((int)dm) * 4);   // y: after out_proj
+    w.x8 = nullptr;
+    w.x_inv = nullptr;
+    if (i8) {
+        // their own blocks: x8 lives from norm2 (or the stack input's quantise pass) to the next QKV projection, which writes
+        // qkv and so cannot share it, while the other buffers it could share are not provably as large for every shape
+        w.x8 = b.take<int8_t>(rows * dm);
+        w.x_inv = b.take<float>(rows * 4);
+    }
     return w;
 }
 
@@ -612,7 +724,7 @@ std::unique_ptr<ForwardPlan> TxModel::make_plan(int N, int T_in, const __half* s
     const Shapes s = shapes(T_in);
     const int T = s.t.back();
     Bump b(ws, ws_bytes);
-    const auto [cbuf, x, y, att, qkv, hid, ups, ss_a, ss_b] = carve(b, N, T_in);
+    const auto [cbuf, x, y, att, qkv, hid, ups, ss_a, ss_b, x8, x_inv] = carve(b, N, T_in);
     if (b.used() != ws_bytes) throw std::logic_error("tx workspace: the plan's layout differs from workspace_bytes()");
     auto plan = std::make_unique<TxPlan>();
     const long long rows = (long long)N * T;
@@ -673,7 +785,23 @@ std::unique_ptr<ForwardPlan> TxModel::make_plan(int N, int T_in, const __half* s
     for (int l = 0; l < desc.depth; ++l) {
         const auto& lw = layers[l];
         TxPlan::Layer L;
-        if (fp8) {
+        if (i8) {
+            // x holds the normalised rows (the conv output before layer 0) and x8 / x_inv their int8 copy.  qkv: int8 x int8
+            // with RoPE; out_proj -> y (+ alpha * x); norm1 y -> att (fp16) + qkv's buffer (E4M3); fc1 + SwiGLU -> hid
+            // (E4M3); fc2 -> y (+ alpha * att); norm2 y -> x (fp16) + x8 / x_inv
+            GemmDesc q = dense(x8, dm, lw.wqkv_i8, dqkv, nullptr, GEMM_ACT_ROPE, qkv, dqkv, nullptr, 0.0f);
+            q.q8 = GEMM_Q8_OPERANDS;
+            q.row_scale = x_inv;
+            q.col_scale = lw.wqkv_inv;
+            L.qkv = make_gemm_plan(q);
+            L.out_proj = make_gemm_plan(dense(att, dm, lw.wo, dm, lw.bo, GEMM_ACT_NONE, y, dm, x, desc.deepnorm_alpha));
+            GemmDesc f1 = dense(qkv, dm, lw.w1_e4m3, 2 * ff, nullptr, GEMM_ACT_SWIGLU, hid, ff, nullptr, 0.0f);
+            f1.fp8 = 1;
+            L.fc1 = make_gemm_plan(f1);
+            GemmDesc f2 = dense(hid, ff, lw.w2_e4m3, dm, nullptr, GEMM_ACT_NONE, y, dm, att, desc.deepnorm_alpha);
+            f2.fp8 = 1;
+            L.fc2 = make_gemm_plan(f2);
+        } else if (fp8) {
             // qkv and out_proj as in the folded fp16 layout; norm1 -> att (fp16) + qkv's buffer (E4M3, free once attention has
             // read it); fc1 + SwiGLU -> hid (E4M3); fc2 -> x (fp16, + alpha * att) with the partial sums for the folded norm2
             const bool first = l == 0;
@@ -749,9 +877,12 @@ std::unique_ptr<ForwardPlan> TxModel::make_plan(int N, int T_in, const __half* s
     plan->norm_dim = dm;
     plan->fold_norm = fold_norm;
     plan->fp8 = fp8;
+    plan->i8 = i8;
     plan->norm_out = att;
     plan->norm_out8 = reinterpret_cast<uint8_t*>(qkv);
-    plan->n_launches = 1 + (desc.num_convs - 1) + desc.depth * (fp8 ? 6 : fold_norm ? 5 : 7) + 2;
+    plan->x8 = x8;
+    plan->x_inv = x_inv;
+    plan->n_launches = 1 + (desc.num_convs - 1) + (i8 ? 1 : 0) + desc.depth * (i8 ? 7 : fp8 ? 6 : fold_norm ? 5 : 7) + 2;
     if (const char* dbg = std::getenv("B200_DEBUG_TX_LAUNCHES")) {   // debug: stop after k launches (tests/test_tx_layers_gpu.py)
         const int k = std::atoi(dbg);
         if (k >= 0 && k < plan->n_launches) plan->stop_after = k;
@@ -780,6 +911,11 @@ void TxPlan::run(cudaStream_t stream, ProfileSink* prof) {
         }
     }
     const unsigned norm_grid = (unsigned)((rows + 7) / 8);
+    if (i8) {
+        NvtxRange r("Quantise I8");
+        quantize_i8_kernel<<<norm_grid, 256, 0, stream>>>(x, rows, norm_dim, x8, x_inv);
+        if (done("quantize_i8")) return;
+    }
     {
         NvtxRange enc("TransEnc");
         for (auto& L : layers) {
@@ -801,11 +937,11 @@ void TxPlan::run(cudaStream_t stream, ProfileSink* prof) {
             }
             if (fp8) {
                 NvtxRange r("LNORM1");
-                rmsnorm_kernel<<<norm_grid, 256, 0, stream>>>(y, norm_out, L.n1, rows, norm_dim, norm_out8);
+                rmsnorm_kernel<<<norm_grid, 256, 0, stream>>>(y, norm_out, L.n1, rows, norm_dim, norm_out8, nullptr, nullptr);
                 if (done("rmsnorm_e4m3")) return;
             } else if (!fold_norm) {
                 NvtxRange r("LNORM1");
-                rmsnorm_kernel<<<norm_grid, 256, 0, stream>>>(y, x, L.n1, rows, norm_dim, nullptr);
+                rmsnorm_kernel<<<norm_grid, 256, 0, stream>>>(y, x, L.n1, rows, norm_dim, nullptr, nullptr, nullptr);
                 if (done("rmsnorm")) return;
             }
             {
@@ -820,8 +956,8 @@ void TxPlan::run(cudaStream_t stream, ProfileSink* prof) {
             }
             if (!fold_norm) {
                 NvtxRange r("LNORM2");
-                rmsnorm_kernel<<<norm_grid, 256, 0, stream>>>(y, x, L.n2, rows, norm_dim, nullptr);
-                if (done("rmsnorm")) return;
+                rmsnorm_kernel<<<norm_grid, 256, 0, stream>>>(y, x, L.n2, rows, norm_dim, nullptr, x8, x_inv);   // x8: int8_qkv only
+                if (done(i8 ? "rmsnorm_i8" : "rmsnorm")) return;
             }
         }
     }
@@ -890,6 +1026,29 @@ uint8_t e4m3_from_f16_bits(uint16_t b) {
     const uint32_t rest = u & 0xfffffu;
     if (rest > 0x80000u || (rest == 0x80000u && (keep & 1u))) ++keep;
     return sign | (uint8_t)(keep - ((127u - 7u) << 3));
+}
+
+void test_quantize_act_rows_host(int device, const uint16_t* f16, int rows, int cols, int8_t* q, float* inv) {
+    if (rows < 1 || cols < 128 || cols % 128 != 0 || (long long)rows * cols >= (1LL << 40)) {
+        throw std::invalid_argument("test_quantize_act_rows: rows >= 1 and cols a positive multiple of 128");
+    }
+    require_sm90(device);
+    const size_t n = (size_t)rows * cols;
+    __half* d_in = nullptr;
+    int8_t* d_q = nullptr;
+    float* d_inv = nullptr;
+    Arena arena;
+    arena.allocate([&](Bump& b) {
+        d_in = b.take<__half>(n * 2);
+        d_q = b.take<int8_t>(n);
+        d_inv = b.take<float>((size_t)rows * 4);
+    });
+    B200_CUDA(cudaMemcpy(d_in, f16, n * 2, cudaMemcpyHostToDevice));
+    quantize_i8_kernel<<<(unsigned)((rows + 7) / 8), 256>>>(d_in, rows, cols, d_q, d_inv);
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaDeviceSynchronize());
+    B200_CUDA(cudaMemcpy(q, d_q, n, cudaMemcpyDeviceToHost));
+    B200_CUDA(cudaMemcpy(inv, d_inv, (size_t)rows * 4, cudaMemcpyDeviceToHost));
 }
 
 void test_attention_host(int device, const uint16_t* qkv, int N, int T, int H, int win_upper, int win_lower, uint16_t* out) {

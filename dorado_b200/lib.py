@@ -47,7 +47,7 @@ class ModelDesc(C.Structure):
 
 
 # precision name -> (b200_model_desc.tx_precision, b200_model_desc.lstm_precision)
-PRECISIONS = {"fp16": (0, 0), "fp8_ffn": (1, 0), "int8_lstm": (0, 1)}
+PRECISIONS = {"fp16": (0, 0), "fp8_ffn": (1, 0), "int8_qkv_fp8_ffn": (2, 0), "int8_lstm": (0, 1)}
 
 
 class Tensor(C.Structure):
@@ -112,7 +112,7 @@ EXPORTS = [
     "b200_runner_set_decoder_options", "b200_runner_batch_size", "b200_runner_chunk_size", "b200_runner_out_len",
     "b200_runner_accept_chunk_f16", "b200_runner_accept_chunk_f32", "b200_runner_input", "b200_runner_call_chunks",
     "b200_runner_upload", "b200_runner_step_device", "b200_runners_step_device", "b200_runner_forward_scores", "b200_runner_profile", "b200_runner_plan_info", "b200_runner_debug_read_workspace", "b200_decode_scores",
-    "b200_test_gemm", "b200_test_gemm_desc", "b200_test_gemm_fp8", "b200_test_gemm_s8", "b200_test_quantize_rows", "b200_test_to_e4m3", "b200_test_remove_bits", "b200_test_attention", "b200_generate_chunks", "b200_stitch_chunks", "b200_runner_accept_raw_chunk",
+    "b200_test_gemm", "b200_test_gemm_desc", "b200_test_gemm_fp8", "b200_test_gemm_s8", "b200_test_gemm_s8_scaled", "b200_test_quantize_act_rows", "b200_test_quantize_rows", "b200_test_to_e4m3", "b200_test_remove_bits", "b200_test_attention", "b200_generate_chunks", "b200_stitch_chunks", "b200_runner_accept_raw_chunk",
     "b200_runner_debug_read_input", "b200_engine_runner_bytes", "b200_engine_benchmark_batch_sizes",
     "b200_select_batch_size", "b200_generate_variable_chunks", "b200_engine_terminate", "b200_engine_restart",
     "b200_engine_set_low_latency", "b200_engine_is_low_latency", "b200_engine_batch_timeouts_ms",
@@ -201,6 +201,8 @@ def load_library() -> C.CDLL:
     lib.b200_test_gemm_fp8.argtypes = [i32, vp, vp, i32, i32, i32, i32, vp, f32, vp]
     lib.b200_test_gemm_s8.argtypes = [i32, vp, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.b200_test_quantize_rows.argtypes = [vp, i32, i32, vp, vp]
+    lib.b200_test_gemm_s8_scaled.argtypes = [i32, vp, vp, vp, vp, i32, i32, i32, i32, f32, i32, i32, i32, vp]
+    lib.b200_test_quantize_act_rows.argtypes = [i32, vp, i32, i32, vp, vp]
     lib.b200_test_to_e4m3.argtypes = [vp, C.c_int64, vp]
     lib.b200_test_remove_bits.argtypes = [vp, C.c_int64, i32, vp]
     u64 = C.c_uint64
@@ -233,8 +235,9 @@ def check(status: int) -> None:
 
 
 def model_desc_from_config(cfg: BasecallModelConfig, precision: str = "fp16") -> ModelDesc:
-    """precision: "fp16" (default), "fp8_ffn" (transformer models: E4M3 feed-forward GEMMs) or "int8_lstm" (LSTM models
-    of lstm_size 256 / 384: int8 LSTM layers and CRF linear); see tx_precision and lstm_precision in b200call.h."""
+    """precision: "fp16" (default), "fp8_ffn" (transformer models: E4M3 feed-forward GEMMs), "int8_qkv_fp8_ffn"
+    (transformer models: fp8_ffn with an int8 QKV projection, the reference's default on an H100) or "int8_lstm" (LSTM
+    models of lstm_size 256 / 384: int8 LSTM layers and CRF linear); see tx_precision and lstm_precision in b200call.h."""
     if precision not in PRECISIONS:
         raise ValueError(f"precision must be one of {sorted(PRECISIONS)}, got {precision!r}")
     d = ModelDesc()
@@ -379,6 +382,36 @@ def test_gemm_s8(a: np.ndarray, b: np.ndarray, col_scale: np.ndarray, bias: np.n
     check(lib.b200_test_gemm_s8(device, a.ctypes.data, b.ctypes.data, col_scale.ctypes.data, bias_p, M, N, K, activation,
                                 c.ctypes.data))
     return c
+
+
+def test_gemm_s8_scaled(a: np.ndarray, b: np.ndarray, row_scale: np.ndarray, col_scale: np.ndarray, activation: int = -1,
+                       theta: float = 0.0, max_seq_len: int = 0, rope_T: int = 0, rope_cols: int = 0, device: int = 0):
+    """The int8 GEMM with per-row and per-column factors on host data: a [M, K], b [N, K] int8 -> fp16 [M, N] of
+    (float(a b^T) * row_scale[m]) * col_scale[n], with RoPE at position m % rope_T on the first rope_cols columns when
+    activation is 5 (b200_test_gemm_s8_scaled)."""
+    lib = load_library()
+    a = np.ascontiguousarray(a, np.int8)
+    b = np.ascontiguousarray(b, np.int8)
+    M, K = a.shape
+    N = b.shape[0]
+    row_scale = np.ascontiguousarray(row_scale, np.float32)
+    col_scale = np.ascontiguousarray(col_scale, np.float32)
+    assert row_scale.shape == (M,) and col_scale.shape == (N,)
+    c = np.empty((M, N), np.float16)
+    check(lib.b200_test_gemm_s8_scaled(device, a.ctypes.data, b.ctypes.data, row_scale.ctypes.data, col_scale.ctypes.data, M, N,
+                                       K, activation, theta, max_seq_len, rope_T, rope_cols, c.ctypes.data))
+    return c
+
+
+def quantize_act_rows(x: np.ndarray, device: int = 0):
+    """The int8_qkv_fp8_ffn device quantiser on host fp16 rows [rows, cols] (cols a multiple of 128): (int8 [rows, cols],
+    fp32 inv [rows])."""
+    h = np.ascontiguousarray(x, np.float16)
+    q = np.empty(h.shape, np.int8)
+    inv = np.empty(h.shape[0], np.float32)
+    check(load_library().b200_test_quantize_act_rows(device, h.ctypes.data, h.shape[0], h.shape[1], q.ctypes.data,
+                                                      inv.ctypes.data))
+    return q, inv
 
 
 def quantize_rows(w: np.ndarray):

@@ -37,8 +37,9 @@ class B200Caller:
 
     def __init__(self, cfg: BasecallModelConfig, weights: dict, device: int = 0, low_latency: bool = False,
                  num_runners: int = 2, precision: str = "fp16"):
-        """precision: "fp16", "fp8_ffn" (transformer models: fc1 / fc2 on E4M3 operands) or "int8_lstm" (LSTM models of
-        lstm_size 256 / 384: int8 LSTM layers and CRF linear); include/b200call.h."""
+        """precision: "fp16", "fp8_ffn" (transformer models: fc1 / fc2 on E4M3 operands), "int8_qkv_fp8_ffn" (transformer
+        models: fp8_ffn with the QKV projection on int8 operands) or "int8_lstm" (LSTM models of lstm_size 256 / 384: int8
+        LSTM layers and CRF linear); include/b200call.h."""
         self.cfg = cfg
         self.device = device
         self.precision = precision

@@ -71,10 +71,12 @@ public:
             d.upsample_scale = model_config.tx->upsample.scale_factor;
             d.tx_crf_scale = model_config.tx->crf.scale;
             // The reference's dev option (TxModules.cpp:477-479): koi_use_f8=1 runs fc1 / fc2 on E4M3 operands with
-            // remove_bits = 4 on the fp16 weights it keeps (b200call.h, tx_precision).  Off unless asked for here: the fp16
-            // path is the one held to the oracle.  koi_use_i8 and other remove_bits values have no counterpart.
+            // remove_bits = 4 on the fp16 weights it keeps (b200call.h, tx_precision).  Together with an explicit koi_use_i8=1
+            // (TxModules.cpp:936), the reference's default on an H100, the QKV projection also runs on int8 operands.  Off
+            // unless asked for here: the fp16 path is the one held to the oracle.  koi_use_i8 without koi_use_f8 (int8 fc1)
+            // and other remove_bits values have no counterpart, and leave the model in fp16.
             if (utils::get_dev_opt<bool>("koi_use_f8", false)) {
-                d.tx_precision = B200_TX_FP8_FFN;
+                d.tx_precision = utils::get_dev_opt<bool>("koi_use_i8", false) ? B200_TX_I8_QKV_FP8_FFN : B200_TX_FP8_FFN;
             }
         }
         // The reference's own override (ConvStack.cpp:77-87): DORADO_LSTM_MODE=CUTLASS_TNC_I8 selects the int8 LSTM layers

@@ -38,7 +38,7 @@ enum { B200_ACT_SWISH = 0, B200_ACT_SWISH_CLAMP = 1, B200_ACT_TANH = 2 };
 /* model family */
 enum { B200_MODEL_LSTM = 0, B200_MODEL_TX = 1 };
 /* transformer precision (b200_model_desc.tx_precision) */
-enum { B200_TX_FP16 = 0, B200_TX_FP8_FFN = 1 };
+enum { B200_TX_FP16 = 0, B200_TX_FP8_FFN = 1, B200_TX_I8_QKV_FP8_FFN = 2 };
 /* LSTM precision (b200_model_desc.lstm_precision) */
 enum { B200_LSTM_FP16 = 0, B200_LSTM_INT8 = 1 };
 
@@ -82,7 +82,14 @@ typedef struct b200_model_desc {
      * scale.  norm1 writes its output in fp16 and as an E4M3 copy, fc1 + SwiGLU reads the copy and writes E4M3, fc2 reads
      * that and writes fp16; both accumulate in fp32.  Shapes: those above, and dim_feedforward a multiple of 128 (fc2's K
      * in whole 128-byte E4M3 blocks; the engine does not pad it): others return B200_ERR_UNSUPPORTED.  On an LSTM model,
-     * or any other value, b200_engine_create returns B200_ERR_INVALID.  b200_runner_plan_info reports "tx.fp8_ffn=1". */
+     * or any other value, b200_engine_create returns B200_ERR_INVALID.  b200_runner_plan_info reports "tx.fp8_ffn=1".
+     * B200_TX_I8_QKV_FP8_FFN (2): koi_use_f8 = 1 with koi_use_i8 = 1, the reference's default on an H100
+     * (TxModules.cpp:477-479, 936-961, 497-506, 611-616, 669, 713).  As B200_TX_FP8_FFN, and the fused QKV + RoPE projection
+     * takes int8 operands: Wqkv is quantised per output row from the fp16 weights before remove_bits
+     * (utils::quantize_tensor, evaluated in fp16), the encoder stack's input per token row by a device pass, and norm2 becomes
+     * an explicit pass that writes the next layer's fp16 rows and their int8 copy; the s32 accumulator is converted to fp32
+     * and multiplied by the row's and then the column's factor 1 / scale.  The same shapes and errors as B200_TX_FP8_FFN.
+     * b200_runner_plan_info reports "tx.fp8_ffn=1;tx.int8_qkv=1". */
     int32_t tx_precision;
     /* LSTM precision.  B200_LSTM_FP16 (0, what a zero-initialised descriptor gets): fp16 operands, fp32 accumulation.
      * B200_LSTM_INT8 (1): the reference's CUTLASS_TNC_I8 layout (dorado/nn/ConvStack.cpp:66-74, LSTMStack.cpp:127-211,
@@ -513,6 +520,18 @@ B200_API int b200_test_gemm_fp8(int32_t device, const uint8_t* a, const uint8_t*
  * bias may be NULL. */
 B200_API int b200_test_gemm_s8(int32_t device, const int8_t* a, const int8_t* b, const float* col_scale, const float* bias,
                                int32_t M, int32_t N, int32_t K, int32_t activation, uint16_t* c);
+/* The GEMM with int8 operands and per-row and per-column factors (A [M,K], W [N,K]; K is zero-padded to a multiple of 128
+ * inside; N a multiple of 32): v = (float(A W^T) * row_scale[m]) * col_scale[n], each product rounded in fp32, the s32 -> fp32
+ * conversion to nearest even.  activation -1: c = fp16(v) [M,N].  activation 5 (RoPE, the int8_qkv_fp8_ffn QKV projection):
+ * the first rope_cols columns (whole 64-column heads) rotated at position m % rope_T with the model's fp32 table for theta
+ * and max_seq_len positions (1 <= rope_T <= max_seq_len), then fp16; the theta and rope arguments are ignored otherwise. */
+B200_API int b200_test_gemm_s8_scaled(int32_t device, const int8_t* a, const int8_t* b, const float* row_scale,
+                                      const float* col_scale, int32_t M, int32_t N, int32_t K, int32_t activation, float theta,
+                                      int32_t max_seq_len, int32_t rope_T, int32_t rope_cols, uint16_t* c);
+/* The int8_qkv_fp8_ffn precision's device quantiser on fp16 rows [rows, cols] (cols a positive multiple of 128): int8 q
+ * [rows, cols] and fp32 inv [rows] = 1 / float(fp16(128 / absmax)), bit for bit b200_test_quantize_rows' q and the reciprocal
+ * of its scale (0 where the scale is +inf). */
+B200_API int b200_test_quantize_act_rows(int32_t device, const uint16_t* f16, int32_t rows, int32_t cols, int8_t* q, float* inv);
 /* Host only, no device: the int8_lstm weight quantisation of fp16 values [rows, cols], per row, as utils::quantize_tensor(w, 1)
  * computes it on an fp16 tensor: scale = fp16(128 / absmax), q = clip(round_half_even(fp16(w * scale)), -127, 127).  An all-zero
  * row gets q = 0 and scale = +inf (the engine dequantises such a row with the factor 0). */

@@ -2,11 +2,13 @@
 """Throughput of the transformer models on one GPU: sup@v5 (d_model 512, window (127, 128)) and the synthetic 1536-wide
 fixture (d_model 1536, 24 heads, window (255, 256), feed-forward 6144; see tests/test_tx1536_cpu.py).
 
-usage: python tools/bench_tx.py --model sup|tx1536 [--precision fp16|fp8_ffn] [--batch 128] [--chunksize 12288]
+usage: python tools/bench_tx.py --model sup|tx1536 [--precision fp16|fp8_ffn|int8_qkv_fp8_ffn] [--batch 128] [--chunksize 12288]
        [--runners 2] [--steps 10] [--warmup 3]
 
 --precision fp8_ffn runs fc1 + SwiGLU and fc2 on E4M3 operands behind an explicit norm1 pass (include/b200call.h); their
-FLOP rates are then to be read against the data sheet's dense FP8 figure (1,979 TFLOP/s), also printed.
+FLOP rates are then to be read against the data sheet's dense FP8 figure (1,979 TFLOP/s), also printed.  --precision
+int8_qkv_fp8_ffn also runs the QKV projection on int8 operands (the data sheet's dense INT8 figure is 1,979 TOPS), behind a
+quantise pass of the stack's input and an explicit norm2 pass that writes the int8 copy.
 
 Device-resident steps as bench.py times them (step i on runner i % R, each runner on its own stream), then one profiled
 forward + decode with an event after every launch.  Prints one JSON line: samples/s, the card (name, power limit, SM
@@ -77,7 +79,7 @@ def main():
     from dorado_b200.weights import synthetic_weights
     ap = argparse.ArgumentParser()
     ap.add_argument("--model", required=True, choices=list(MODELS))
-    ap.add_argument("--precision", default="fp16", choices=["fp16", "fp8_ffn"])
+    ap.add_argument("--precision", default="fp16", choices=["fp16", "fp8_ffn", "int8_qkv_fp8_ffn"])
     ap.add_argument("--batch", type=int, default=128)
     ap.add_argument("--chunksize", type=int, default=12288)
     ap.add_argument("--runners", type=int, default=2)
@@ -113,10 +115,12 @@ def main():
         if k in prof:
             launches, t = prof[k]
             rates[k] = {"ms_per_launch": t / launches, "tflops": f * rows * launches / (t * 1e-3) / 1e12}
-    if "rmsnorm_e4m3" in prof:   # reads the fp16 row, writes it in fp16 and E4M3
-        launches, t = prof["rmsnorm_e4m3"]
-        rates["rmsnorm_e4m3"] = {"ms_per_launch": t / launches,
-                                 "gb_per_s": rows * cfg.tx.d_model * 5 * launches / (t * 1e-3) / 1e9}
+    # bytes per element: rmsnorm_e4m3 reads the fp16 row, writes it in fp16 and E4M3; rmsnorm_i8 also reads its fp16 output
+    # back and writes int8; quantize_i8 reads fp16 and writes int8
+    for k, per_elem in (("rmsnorm_e4m3", 5), ("rmsnorm_i8", 7), ("quantize_i8", 3)):
+        if k in prof:
+            launches, t = prof[k]
+            rates[k] = {"ms_per_launch": t / launches, "gb_per_s": rows * cfg.tx.d_model * per_elem * launches / (t * 1e-3) / 1e9}
     att_launches, att_ms = prof["tx_attention"]
     fps = flop_per_sample(cfg)
     out = {"model": args.model, "precision": args.precision, "d_model": cfg.tx.d_model, "nhead": cfg.tx.nhead, "attn_window": list(cfg.tx.attn_window),
