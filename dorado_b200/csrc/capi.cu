@@ -398,44 +398,10 @@ int b200_decode_scores(int32_t device, const uint16_t* scores, int32_t N, int32_
     });
 }
 
-int b200_test_gemm(int32_t device, const uint16_t* a, const uint16_t* b, const float* bias, int32_t M, int32_t N,
-                   int32_t K, int32_t activation, uint16_t* c) {
-    return guarded([&] {
-        if (!a || !b || !c) throw std::invalid_argument("b200_test_gemm: null argument");
-        b200::test_gemm_host(device, a, b, bias, M, N, K, activation, c);
-    });
-}
-
 int b200_test_gemm_desc(int32_t device, const b200_gemm_test_desc* desc) {
     return guarded([&] {
         if (!desc) throw std::invalid_argument("b200_test_gemm_desc: null argument");
         b200::test_gemm_desc_host(device, *desc);
-    });
-}
-
-int b200_test_gemm_fp8(int32_t device, const uint8_t* a, const uint8_t* b, int32_t M, int32_t N, int32_t K, int32_t activation,
-                       const uint16_t* residual, float alpha, void* c) {
-    return guarded([&] {
-        if (!a || !b || !c) throw std::invalid_argument("b200_test_gemm_fp8: null argument");
-        b200::test_gemm_fp8_host(device, a, b, M, N, K, activation, residual, alpha, c);
-    });
-}
-
-int b200_test_gemm_s8(int32_t device, const int8_t* a, const int8_t* b, const float* col_scale, const float* bias, int32_t M,
-                      int32_t N, int32_t K, int32_t activation, uint16_t* c) {
-    return guarded([&] {
-        if (!a || !b || !col_scale || !c) throw std::invalid_argument("b200_test_gemm_s8: null argument");
-        b200::test_gemm_s8_host(device, a, b, col_scale, bias, M, N, K, activation, c);
-    });
-}
-
-int b200_test_gemm_s8_scaled(int32_t device, const int8_t* a, const int8_t* b, const float* row_scale, const float* col_scale,
-                             int32_t M, int32_t N, int32_t K, int32_t activation, float theta, int32_t max_seq_len,
-                             int32_t rope_T, int32_t rope_cols, uint16_t* c) {
-    return guarded([&] {
-        if (!a || !b || !row_scale || !col_scale || !c) throw std::invalid_argument("b200_test_gemm_s8_scaled: null argument");
-        b200::test_gemm_s8_scaled_host(device, a, b, row_scale, col_scale, M, N, K, activation, theta, max_seq_len, rope_T,
-                                       rope_cols, c);
     });
 }
 

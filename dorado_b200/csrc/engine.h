@@ -372,20 +372,10 @@ private:
 void decode_host_scores(int device, const uint16_t* scores, int N, int T, int C, float clamp_val,
                         const b200_decoder_options& opts, uint8_t* moves, char* sequence, char* qstring,
                         int32_t* n_bases);
-void test_gemm_host(int device, const uint16_t* a, const uint16_t* b, const float* bias, int M, int N, int K,
-                    int activation, uint16_t* c);
 void test_gemm_desc_host(int device, const b200_gemm_test_desc& t);
 // The transformer's rotary table (tx_model.cu): [16 dim pairs][tmax positions] float4 (cos, sin, cos, sin), in fp32
 std::vector<float> rope_table(float theta, int tmax);
 void test_attention_host(int device, const uint16_t* qkv, int N, int T, int H, int win_upper, int win_lower, uint16_t* out);
-void test_gemm_fp8_host(int device, const uint8_t* a, const uint8_t* b, int M, int N, int K, int activation,
-                        const uint16_t* residual, float alpha, void* c);
-
-void test_gemm_s8_host(int device, const int8_t* a, const int8_t* b, const float* col_scale, const float* bias, int M, int N,
-                       int K, int activation, uint16_t* c);
-void test_gemm_s8_scaled_host(int device, const int8_t* a, const int8_t* b, const float* row_scale, const float* col_scale,
-                              int M, int N, int K, int activation, float theta, int max_seq_len, int rope_T, int rope_cols,
-                              uint16_t* c);
 // The int8_qkv_fp8_ffn transformer's device quantiser (tx_model.cu) on host fp16 rows [rows][cols] (cols a multiple of
 // 128): int8 rows and the fp32 factor 1 / float(scale16) of each, bit for bit quantize_rows_f16's values
 void test_quantize_act_rows_host(int device, const uint16_t* f16, int rows, int cols, int8_t* q, float* inv);

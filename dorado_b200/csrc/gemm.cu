@@ -8,12 +8,13 @@
 // A and W tiles, 128-byte swizzle, a STAGES-deep mbarrier ring that runs across tiles); warpgroups 1 and 2 own rows 0-63 and
 // 64-127 of the tile: they issue wgmma m64n32k16 straight from the swizzled stages, keep the fp32 accumulator in registers
 // and run the epilogue (bias / activation / residual / rotary / SwiGLU -> fp16 -> global) from the accumulator fragments.
-// E4M3 form (template FP8, the transformer's fc1 / fc2 in the fp8_ffn precision): the same ring, tiles and epilogues with
-// 128 E4M3 per 128-byte K row instead of 64 fp16, wgmma m64n32k32.e4m3 and the SwiGLU output cast to E4M3.
-// int8 form (template Q8 = GEMM_Q8_OPERANDS, the x-projection and the CRF linear of LSTM models in the int8_lstm precision):
-// the E4M3 form's ring and boxes, wgmma m64n32k32.s8 into s32 accumulators, which the epilogue converts and multiplies by a
-// per-column fp32 factor (and a per-row one with row_scale: the transformer's QKV + RoPE projection in the int8_qkv_fp8_ffn
-// precision).  Q8 = GEMM_Q8_STORE is the fp16 form whose tanh epilogue stores int8 (those models' last conv).
+// The kernel's template names its form: activation, operand type, output type and row factors (kForms below lists the 14
+// forms that are built).  E4M3 operands (the transformer's fc1 / fc2 in the fp8_ffn precision): the same ring, tiles and
+// epilogues with 128 E4M3 per 128-byte K row instead of 64 fp16, wgmma m64n32k32.e4m3 and the SwiGLU output cast to E4M3.
+// int8 operands (the x-projection and the CRF linear of LSTM models in the int8_lstm precision): the E4M3 form's ring and
+// boxes, wgmma m64n32k32.s8 into s32 accumulators, which the epilogue converts and multiplies by a per-column fp32 factor
+// (and by a per-row one in the forms with row factors: the transformer's QKV + RoPE projection in the int8_qkv_fp8_ffn
+// precision).  The int8 output goes with fp16 operands: the tanh epilogue stores int8 (those models' last conv).
 // A is addressed through a 3-D tensor map (k, row, batch) so that overlapping-row views work: the last conv of the LSTM
 // models reads its im2col rows straight from the NTC activation buffer with row stride = stride * C_in (the reference's
 // "cutlass_conv" trick, ConvStack.cpp:236-275).
@@ -34,15 +35,12 @@ namespace b200 {
 namespace {
 
 constexpr int BM = 128;
-constexpr int BK = 64;              // fp16 per K block: one 128-byte swizzle row (128 E4M3 in the fp8 form)
-constexpr int BK8 = 128;
+constexpr int BK = 64;              // fp16 per K block: one 128-byte swizzle row
+constexpr int BK8 = 128;            // E4M3 or int8 per K block
 constexpr int BN_MAX = 128;
 constexpr int STAGES = 5;          // TMA -> wgmma ring depth: 5 x 32 KB of the 227 KB
 constexpr int GEMM_PARTS = 4;      // RMSNorm partial sums per row and column tile (GemmDesc::out_ss): one per 32-column chunk
 constexpr int GEMM_THREADS = 384;  // warpgroup 0: producer; warpgroups 1, 2: MMA + epilogue of 64 rows each
-// Kernel form (template Q8) of GEMM_Q8_OPERANDS with GemmDesc::row_scale: its own instantiations, so that the int8 forms
-// without row factors keep their code
-constexpr int Q8_OPERANDS_ROWS = 3;
 
 struct GemmKernelParams {
     int rows_per_batch, tiles_per_batch, N, num_k_blocks, bn;
@@ -63,8 +61,8 @@ struct GemmKernelParams {
     const float* res_gain;
     int a_ss_parts, res_ss_parts;
     float norm_inv_dim, norm_eps;
-    const float* col_scale;   // GEMM_Q8_OPERANDS
-    const float* row_scale;   // GEMM_Q8_OPERANDS, optional
+    const float* col_scale;   // int8 operands
+    const float* row_scale;   // int8 operands, the forms with row factors
 };
 
 // i-th tile of this CTA: row tile mt, column tile nt; false when the CTA has run out of tiles.  Producer and consumers walk
@@ -112,12 +110,14 @@ __device__ __forceinline__ void wgmma_k_block(Acc (&acc)[BN_MAX / 32][16], uint6
     }
 }
 
-template <int ACT, bool FP8, int Q8 = GEMM_Q8_NONE>
+// ROWS: int8 operands with per-row factors (GemmDesc::row_scale), their own forms so that those without keep their code
+template <int ACT, GemmType IN, GemmType OUT, bool ROWS>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a,
                                                                      const __grid_constant__ CUtensorMap tma_w,
                                                                      const GemmKernelParams p) {
-    constexpr bool ROWS = Q8 == Q8_OPERANDS_ROWS;
-    constexpr bool S8 = Q8 == GEMM_Q8_OPERANDS || ROWS;
+    constexpr bool FP8 = IN == GEMM_E4M3;
+    constexpr bool S8 = IN == GEMM_S8;
+    constexpr bool STORE_S8 = OUT == GEMM_S8;   // fp16 operands, int8 output
     constexpr int KB = FP8 || S8 ? BK8 : BK;   // K elements per block
     using Acc = std::conditional_t<S8, int32_t, float>;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -343,7 +343,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                                 ss_out[h][c] = fmaf(f.x, f.x, ss_out[h][c]);
                                 ss_out[h][c] = fmaf(f.y, f.y, ss_out[h][c]);
                             }
-                            if constexpr (Q8 == GEMM_Q8_STORE) {
+                            if constexpr (STORE_S8) {
                                 const int32_t q0 = tc::cvt_rni_sat_s8(kInt8ActScale * act_apply<ACT>(v0));
                                 const int32_t q1 = tc::cvt_rni_sat_s8(kInt8ActScale * act_apply<ACT>(v1));
                                 *reinterpret_cast<uint16_t*>(reinterpret_cast<int8_t*>(p.out) + off[h] + nc) =
@@ -370,6 +370,75 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
             }
         }
     }
+}
+
+// Optional inputs of a kernel form's epilogue (GemmForm::reads)
+enum : unsigned {
+    READS_BIAS = 1,
+    READS_RESIDUAL = 2,    // residual, res_gain, res_ss
+    READS_A_SS = 4,
+    READS_OUT_SS = 8,
+    READS_COL_SCALE = 16,  // required by the forms that read it
+};
+constexpr unsigned READS_PLAIN = READS_BIAS | READS_RESIDUAL | READS_A_SS | READS_OUT_SS;
+
+using GemmKernel = void (*)(CUtensorMap, CUtensorMap, GemmKernelParams);
+
+// One built instantiation of gemm_wgmma_kernel: the descriptors it runs (types, activation, row_scale set or not) and the
+// optional inputs its epilogue reads
+struct GemmForm {
+    GemmType in, out;
+    int act;
+    bool rows;
+    unsigned reads;
+    GemmKernel kernel;
+};
+
+template <int ACT, GemmType IN, GemmType OUT, bool ROWS = false>
+GemmForm form(unsigned reads) {
+    return {IN, OUT, ACT, ROWS, reads, gemm_wgmma_kernel<ACT, IN, OUT, ROWS>};
+}
+
+const GemmForm kForms[] = {
+        form<GEMM_ACT_NONE, GEMM_F16, GEMM_F16>(READS_PLAIN),
+        form<GEMM_ACT_SWISH, GEMM_F16, GEMM_F16>(READS_PLAIN),
+        form<GEMM_ACT_SWISH_CLAMP, GEMM_F16, GEMM_F16>(READS_PLAIN),
+        form<GEMM_ACT_TANH, GEMM_F16, GEMM_F16>(READS_PLAIN),
+        form<GEMM_ACT_TANH_X5, GEMM_F16, GEMM_F16>(READS_PLAIN),
+        form<GEMM_ACT_SWIGLU, GEMM_F16, GEMM_F16>(READS_BIAS | READS_A_SS),
+        form<GEMM_ACT_ROPE, GEMM_F16, GEMM_F16>(READS_A_SS),
+        form<GEMM_ACT_TANH, GEMM_F16, GEMM_S8>(READS_BIAS),
+        form<GEMM_ACT_NONE, GEMM_E4M3, GEMM_F16>(READS_PLAIN),
+        form<GEMM_ACT_SWIGLU, GEMM_E4M3, GEMM_E4M3>(READS_BIAS | READS_A_SS),
+        form<GEMM_ACT_NONE, GEMM_S8, GEMM_F16>(READS_COL_SCALE | READS_BIAS),
+        form<GEMM_ACT_TANH_X5, GEMM_S8, GEMM_F16>(READS_COL_SCALE | READS_BIAS),
+        form<GEMM_ACT_NONE, GEMM_S8, GEMM_F16, true>(READS_COL_SCALE | READS_BIAS),
+        form<GEMM_ACT_ROPE, GEMM_S8, GEMM_F16, true>(READS_COL_SCALE),
+};
+
+int elem_bytes(GemmType t) { return t == GEMM_F16 ? 2 : 1; }
+
+std::string type_name(GemmType t) {
+    return t == GEMM_F16 ? "fp16" : t == GEMM_E4M3 ? "E4M3" : t == GEMM_S8 ? "int8" : "type " + std::to_string((int)t);
+}
+
+// The descriptor's form, and every input it sets that the form does not read (or col_scale missing where it is required)
+const GemmForm& find_form(const GemmDesc& d) {
+    const std::string what = type_name(d.in_type) + " operands, " + type_name(d.out_type) + " output, activation " +
+                             std::to_string(d.act) + (d.row_scale ? " and row factors" : "");
+    const GemmForm* f = std::find_if(std::begin(kForms), std::end(kForms), [&](const GemmForm& e) {
+        return e.in == d.in_type && e.out == d.out_type && e.act == d.act && e.rows == (d.row_scale != nullptr);
+    });
+    if (f == std::end(kForms)) throw std::invalid_argument("gemm: no kernel form for " + what);
+    const std::pair<unsigned, const char*> inputs[] = {
+            {d.bias ? READS_BIAS : 0u, "bias"}, {d.residual || d.res_gain || d.res_ss ? READS_RESIDUAL : 0u, "residual"},
+            {d.a_ss ? READS_A_SS : 0u, "a_ss"}, {d.out_ss ? READS_OUT_SS : 0u, "out_ss"},
+            {d.col_scale ? READS_COL_SCALE : 0u, "col_scale"}};
+    for (const auto& [given, name] : inputs) {
+        if (given & ~f->reads) throw std::invalid_argument(std::string("gemm: the form for ") + what + " takes no " + name);
+    }
+    if ((f->reads & READS_COL_SCALE) && !d.col_scale) throw std::invalid_argument("gemm: the form for " + what + " needs col_scale");
+    return *f;
 }
 
 using EncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -440,30 +509,16 @@ int gemm_out_ss_parts(int N) {
     return (N / bn) * GEMM_PARTS;
 }
 
-GemmPlan make_gemm_plan(const GemmDesc& d) {
-    const bool s8 = d.q8 == GEMM_Q8_OPERANDS;
-    const int kb = d.fp8 || s8 ? BK8 : BK;
-    const int eb = d.fp8 || s8 ? 1 : 2;   // bytes per A / W element
+namespace {
+
+// Everything make_gemm_plan checks and decides, on the host alone (no driver call): the form, the tile width, the grid,
+// the shared memory.  The tensor maps are left to make_gemm_plan.
+GemmPlan plan_gemm(const GemmDesc& d) {
+    const GemmForm& f = find_form(d);
+    const int eb = elem_bytes(d.in_type);   // bytes per A / W element
+    const int kb = 128 / eb;                // elements per K block: one 128-byte swizzle row
     if (d.K % kb != 0 || d.K <= 0) {
         throw std::invalid_argument(eb == 1 ? "gemm: E4M3 / int8 K must be a positive multiple of 128" : "gemm: K must be a positive multiple of 64");
-    }
-    if (d.q8 != GEMM_Q8_NONE) {
-        const bool plain = !d.fp8 && !d.residual && !d.out_ss && !d.a_ss && !d.res_ss;
-        if (s8 && !d.row_scale && !(plain && d.col_scale && (d.act == GEMM_ACT_NONE || d.act == GEMM_ACT_TANH_X5))) {
-            throw std::invalid_argument("gemm: int8 operands take col_scale, a column bias and the plain or TANH_X5 epilogue only");
-        }
-        if (s8 && d.row_scale && !(plain && d.col_scale && (d.act == GEMM_ACT_NONE || (d.act == GEMM_ACT_ROPE && !d.bias)))) {
-            throw std::invalid_argument("gemm: int8 operands with row_scale take col_scale and the plain (with a column bias) or "
-                                        "the RoPE epilogue (without) only");
-        }
-        if (d.q8 == GEMM_Q8_STORE && !(plain && d.act == GEMM_ACT_TANH)) {
-            throw std::invalid_argument("gemm: the int8 store goes with fp16 operands and the TANH epilogue only");
-        }
-        if (!s8 && d.q8 != GEMM_Q8_STORE) throw std::invalid_argument("gemm: unknown q8 form");
-    }
-    if (d.row_scale && !s8) throw std::invalid_argument("gemm: row_scale goes with int8 operands only");
-    if (d.fp8 && (d.act != GEMM_ACT_NONE && d.act != GEMM_ACT_SWIGLU)) {
-        throw std::invalid_argument("gemm: E4M3 operands take the plain and SwiGLU epilogues only");
     }
     if (d.N % 32 != 0) throw std::invalid_argument("gemm: N must be a multiple of 32");
     if (d.batches < 1 || d.rows_per_batch < 1) throw std::invalid_argument("gemm: empty A");
@@ -472,6 +527,8 @@ GemmPlan make_gemm_plan(const GemmDesc& d) {
     }
     GemmPlan p{};
     p.d = d;
+    p.kernel = reinterpret_cast<const void*>(f.kernel);
+    p.num_k_blocks = d.K / kb;
     p.bn = pick_bn(d.N);
     // few row tiles: split N further to fill more SMs.  Not with out_ss, whose partial slots are laid out for tiles of
     // pick_bn(N) columns (gemm_out_ss_parts); the tile width only changes the occupancy.
@@ -499,6 +556,14 @@ GemmPlan make_gemm_plan(const GemmDesc& d) {
     p.grid = dim3((unsigned)(p.tiles_per_batch * d.batches), (unsigned)(d.N / p.bn), 1);
     p.smem = (size_t)STAGES * ((size_t)BM * 128 + (size_t)p.bn * 128) + 256 + 1024;
     if (p.smem > 227 * 1024) throw std::logic_error("gemm: shared-memory plan does not fit");
+    return p;
+}
+
+}  // namespace
+
+GemmPlan make_gemm_plan(const GemmDesc& d) {
+    GemmPlan p = plan_gemm(d);
+    const uint32_t eb = elem_bytes(d.in_type), kb = 128 / eb;
     const uint64_t batch_stride = d.batches > 1 ? (uint64_t)d.a_batch_stride * eb : (uint64_t)d.a_row_stride * eb * d.rows_per_batch;
     p.tma_a = make_tmap_3d(d.a, (uint64_t)(d.a_inner > 0 ? d.a_inner : d.K), (uint64_t)d.rows_per_batch, (uint64_t)d.batches, (uint64_t)d.a_row_stride * eb,
                            batch_stride, kb, BM, 1, eb);
@@ -506,19 +571,12 @@ GemmPlan make_gemm_plan(const GemmDesc& d) {
     return p;
 }
 
-template <int ACT, bool FP8 = false, int Q8 = GEMM_Q8_NONE>
-static void launch_gemm(int grid, size_t smem, cudaStream_t stream, const CUtensorMap& a, const CUtensorMap& w,
-                        const GemmKernelParams& k) {
-    ensure_dynamic_smem(gemm_wgmma_kernel<ACT, FP8, Q8>, 227 * 1024);
-    gemm_wgmma_kernel<ACT, FP8, Q8><<<grid, GEMM_THREADS, smem, stream>>>(a, w, k);
-}
-
 void run_gemm(const GemmPlan& p, cudaStream_t stream) {
     GemmKernelParams k{};
     k.rows_per_batch = p.d.rows_per_batch;
     k.tiles_per_batch = p.tiles_per_batch;
     k.N = p.d.N;
-    k.num_k_blocks = p.d.K / (p.d.fp8 || p.d.q8 == GEMM_Q8_OPERANDS ? BK8 : BK);
+    k.num_k_blocks = p.num_k_blocks;
     k.bn = p.bn;
     k.bias = p.d.bias;
     k.out = static_cast<__half*>(p.d.out);
@@ -547,58 +605,37 @@ void run_gemm(const GemmPlan& p, cudaStream_t stream) {
     k.row_scale = p.d.row_scale;
     const int max_ctas = p.d.max_ctas > 0 && p.d.max_ctas < kNumSMs ? p.d.max_ctas : kNumSMs;
     const int grid = k.num_tiles < max_ctas ? k.num_tiles : max_ctas;
-    if (p.d.fp8) {
-        if (p.d.act == GEMM_ACT_SWIGLU) launch_gemm<GEMM_ACT_SWIGLU, true>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
-        else launch_gemm<GEMM_ACT_NONE, true>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
-        B200_CUDA(cudaGetLastError());
-        return;
-    }
-    if (p.d.q8 != GEMM_Q8_NONE) {
-        if (p.d.q8 == GEMM_Q8_STORE) launch_gemm<GEMM_ACT_TANH, false, GEMM_Q8_STORE>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
-        else if (p.d.act == GEMM_ACT_TANH_X5) launch_gemm<GEMM_ACT_TANH_X5, false, GEMM_Q8_OPERANDS>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
-        else if (p.d.act == GEMM_ACT_ROPE) launch_gemm<GEMM_ACT_ROPE, false, Q8_OPERANDS_ROWS>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
-        else if (p.d.row_scale) launch_gemm<GEMM_ACT_NONE, false, Q8_OPERANDS_ROWS>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
-        else launch_gemm<GEMM_ACT_NONE, false, GEMM_Q8_OPERANDS>(grid, p.smem, stream, p.tma_a, p.tma_w, k);
-        B200_CUDA(cudaGetLastError());
-        return;
-    }
-    switch (p.d.act) {
-        case GEMM_ACT_NONE: launch_gemm<GEMM_ACT_NONE>(grid, p.smem, stream, p.tma_a, p.tma_w, k); break;
-        case GEMM_ACT_SWISH: launch_gemm<GEMM_ACT_SWISH>(grid, p.smem, stream, p.tma_a, p.tma_w, k); break;
-        case GEMM_ACT_SWISH_CLAMP: launch_gemm<GEMM_ACT_SWISH_CLAMP>(grid, p.smem, stream, p.tma_a, p.tma_w, k); break;
-        case GEMM_ACT_TANH: launch_gemm<GEMM_ACT_TANH>(grid, p.smem, stream, p.tma_a, p.tma_w, k); break;
-        case GEMM_ACT_TANH_X5: launch_gemm<GEMM_ACT_TANH_X5>(grid, p.smem, stream, p.tma_a, p.tma_w, k); break;
-        case GEMM_ACT_SWIGLU: launch_gemm<GEMM_ACT_SWIGLU>(grid, p.smem, stream, p.tma_a, p.tma_w, k); break;
-        case GEMM_ACT_ROPE: launch_gemm<GEMM_ACT_ROPE>(grid, p.smem, stream, p.tma_a, p.tma_w, k); break;
-        default: throw std::invalid_argument("gemm: unknown activation");
-    }
+    ensure_dynamic_smem(p.kernel, 227 * 1024);
+    reinterpret_cast<GemmKernel>(p.kernel)<<<grid, GEMM_THREADS, p.smem, stream>>>(p.tma_a, p.tma_w, k);
     B200_CUDA(cudaGetLastError());
 }
 
 // ------------------------------------------------------------------------------------------------
-// test hooks: host buffers in, host buffer out
+// test hook: host buffers in, host buffer out
 // ------------------------------------------------------------------------------------------------
 namespace {
 
 // Refuses, before anything is allocated, a descriptor that would make the kernel read or write outside a buffer of the
-// lengths given (b200_gemm_test_desc).  Ranges first: with rows < 2^31 and strides and offsets < 2^30, every sum below
-// stays under 2^62.
+// lengths given (b200_gemm_test_desc; lengths in elements of each buffer's type).  Ranges first: with rows < 2^31 and
+// strides and offsets < 2^30, every sum below stays under 2^62.
 void check_gemm_test_desc(const b200_gemm_test_desc& t) {
     auto need = [](bool ok, const char* what) {
         if (!ok) throw std::invalid_argument(std::string("b200_test_gemm_desc: ") + what);
     };
     constexpr int64_t kMax = 1LL << 30;
+    need(t.in_type >= GEMM_F16 && t.in_type <= GEMM_S8 && t.out_type >= GEMM_F16 && t.out_type <= GEMM_S8, "unknown element type");
     need(t.batches >= 1 && t.rows_per_batch >= 1 && (int64_t)t.batches * t.rows_per_batch < (1LL << 31), "rows out of range");
     need(t.K >= 1 && t.K <= (1 << 16) && t.N >= 1 && t.N <= (1 << 16), "K or N out of range");
     need(t.a_inner >= 0 && t.a_inner <= t.K, "a_inner must lie in [0, K]");
     need(t.a_row_stride >= 0 && t.a_row_stride < kMax && t.a_batch_stride >= 0 && t.a_batch_stride < kMax, "A strides out of range");
     need(t.out_offset >= 0 && t.out_offset < kMax && t.out_m1 >= 1 && t.out_m1 < kMax && t.out_s0 >= 0 && t.out_s0 < kMax &&
                  t.out_s1 >= 0 && t.out_s1 < kMax, "output addressing out of range");
-    // the epilogue stores column pairs as one 4-byte __half2
+    // the epilogue stores column pairs as one __half2 (two bytes with the int8 output)
     need(t.out_offset % 2 == 0 && t.out_s0 % 2 == 0 && t.out_s1 % 2 == 0, "output offset and strides must be even");
     need(t.a_ss_parts >= 0 && t.a_ss_parts <= 4096 && t.res_ss_parts >= 0 && t.res_ss_parts <= 4096, "partial counts out of range");
     need(t.a_len >= 0 && t.w_len >= 0 && t.bias_len >= 0 && t.residual_len >= 0 && t.res_gain_len >= 0 && t.a_ss_len >= 0 &&
-                 t.res_ss_len >= 0 && t.out_len >= 0 && t.out_ss_len >= 0, "negative buffer length");
+                 t.res_ss_len >= 0 && t.out_len >= 0 && t.out_ss_len >= 0 && t.col_scale_len >= 0 && t.row_scale_len >= 0,
+         "negative buffer length");
     need(t.a && t.w && t.out, "A, W and out are required");
     const int64_t rows = (int64_t)t.batches * t.rows_per_batch;
     // A: the tensor map's extent, (a_inner or K) x rows_per_batch x batches; TMA reads nothing beyond it
@@ -606,6 +643,8 @@ void check_gemm_test_desc(const b200_gemm_test_desc& t) {
     need((t.batches - 1) * t.a_batch_stride + (int64_t)(t.rows_per_batch - 1) * t.a_row_stride + inner <= t.a_len, "A is too short");
     need((int64_t)t.N * t.K <= t.w_len, "W is too short");
     need(!t.bias || t.N <= t.bias_len, "bias is too short");
+    need(!t.col_scale || t.N <= t.col_scale_len, "col_scale is too short");
+    need(!t.row_scale || rows <= t.row_scale_len, "row_scale is too short");
     // out: the largest row offset over g < rows, with non-negative strides at the last g or at the last g of the previous
     // out_m1 block
     const int64_t q = (rows - 1) / t.out_m1, r = (rows - 1) % t.out_m1;
@@ -630,242 +669,102 @@ void check_gemm_test_desc(const b200_gemm_test_desc& t) {
 
 void test_gemm_desc_host(int device, const b200_gemm_test_desc& t) {
     check_gemm_test_desc(t);
-    require_sm90(device);
     const int64_t rows = (int64_t)t.batches * t.rows_per_batch;
     const std::vector<float> rope = t.act == GEMM_ACT_ROPE ? rope_table(t.theta, t.max_seq_len) : std::vector<float>();
-    auto bytes = [](int64_t n, size_t elem) { return (size_t)(n > 0 ? n : 1) * elem; };
-    __half *d_a = nullptr, *d_w = nullptr, *d_res = nullptr, *d_out = nullptr;
-    float *d_bias = nullptr, *d_gain = nullptr, *d_a_ss = nullptr, *d_res_ss = nullptr, *d_out_ss = nullptr, *d_rope = nullptr;
-    Arena arena;
-    arena.allocate([&](Bump& b) {
-        d_a = b.take<__half>(bytes(t.a_len, 2));
-        d_w = b.take<__half>(bytes(t.w_len, 2));
-        d_bias = b.take<float>(bytes(t.bias_len, 4));
-        d_res = b.take<__half>(bytes(t.residual_len, 2));
-        d_gain = b.take<float>(bytes(t.res_gain_len, 4));
-        d_a_ss = b.take<float>(bytes(t.a_ss_len, 4));
-        d_res_ss = b.take<float>(bytes(t.res_ss_len, 4));
-        d_out = b.take<__half>(bytes(t.out_len, 2));
-        d_out_ss = b.take<float>(bytes(t.out_ss_len, 4));
-        d_rope = b.take<float>(bytes((int64_t)rope.size(), 4));
-    });
-    auto up = [](void* dst, const void* src, int64_t n, size_t elem) {
-        if (src && n > 0) B200_CUDA(cudaMemcpy(dst, src, (size_t)n * elem, cudaMemcpyHostToDevice));
-    };
-    up(d_a, t.a, t.a_len, 2);
-    up(d_w, t.w, t.w_len, 2);
-    up(d_bias, t.bias, t.bias_len, 4);
-    up(d_res, t.residual, t.residual_len, 2);
-    up(d_gain, t.res_gain, t.res_gain_len, 4);
-    up(d_a_ss, t.a_ss, t.a_ss_len, 4);
-    up(d_res_ss, t.res_ss, t.res_ss_len, 4);
-    up(d_out, t.out, t.out_len, 2);
-    up(d_rope, rope.data(), (int64_t)rope.size(), 4);
-    if (t.out_ss) B200_CUDA(cudaMemset(d_out_ss, 0xff, bytes(t.out_ss_len, 4)));   // NaN: a partial never written shows
+    // the descriptor on the host buffers first: every refusal of make_gemm_plan comes before any device work
     GemmDesc d{};
-    d.a = d_a;
+    d.in_type = (GemmType)t.in_type;
+    d.out_type = (GemmType)t.out_type;
+    d.col_scale = t.col_scale;
+    d.row_scale = t.row_scale;
+    d.a = t.a;
     d.batches = t.batches;
     d.rows_per_batch = t.rows_per_batch;
     d.a_row_stride = t.a_row_stride;
     d.a_batch_stride = t.a_batch_stride;
     d.a_inner = t.a_inner;
-    d.w = d_w;
+    d.w = t.w;
     d.N = t.N;
     d.K = t.K;
-    d.bias = t.bias ? d_bias : nullptr;
+    d.bias = t.bias;
     d.act = t.act;
-    d.out = d_out + t.out_offset;
+    d.out = t.out;
     d.out_m1 = t.out_m1;
     d.out_s0 = t.out_s0;
     d.out_s1 = t.out_s1;
     if (t.act == GEMM_ACT_ROPE) {
-        d.rope = d_rope;
+        d.rope = rope.data();
         d.rope_T = t.rope_T;
         d.rope_cols = t.rope_cols;
         d.rope_stride = t.max_seq_len;
     }
     d.max_ctas = t.max_ctas;
-    d.residual = t.residual ? d_res : nullptr;
+    d.residual = reinterpret_cast<const __half*>(t.residual);
     d.alpha = t.alpha;
-    d.out_ss = t.out_ss ? d_out_ss : nullptr;
-    d.a_ss = t.a_ss ? d_a_ss : nullptr;
+    d.out_ss = t.out_ss;
+    d.a_ss = t.a_ss;
     d.a_ss_parts = t.a_ss_parts;
-    d.res_ss = t.res_ss ? d_res_ss : nullptr;
+    d.res_ss = t.res_ss;
     d.res_ss_parts = t.res_ss_parts;
-    d.res_gain = t.res_gain ? d_gain : nullptr;
+    d.res_gain = t.res_gain;
     d.norm_dim = t.norm_dim;
     d.norm_eps = t.norm_eps;
-    const GemmPlan plan = make_gemm_plan(d);
-    run_gemm(plan, nullptr);
-    B200_CUDA(cudaDeviceSynchronize());
-    B200_CUDA(cudaMemcpy(t.out, d_out, (size_t)t.out_len * 2, cudaMemcpyDeviceToHost));
-    if (t.out_ss) B200_CUDA(cudaMemcpy(t.out_ss, d_out_ss, (size_t)rows * (t.N / 32) * 4, cudaMemcpyDeviceToHost));
-}
-
-// The dense form: A [M][K], W [N][K], K zero-padded to a multiple of 64 here, c [M][N] (N / 2 with SwiGLU)
-void test_gemm_host(int device, const uint16_t* a, const uint16_t* b, const float* bias, int M, int N, int K, int activation,
-                    uint16_t* c) {
-    if (M < 1 || N < 1 || K < 1) throw std::invalid_argument("test_gemm: empty operand");
-    const int Kp = (K + BK - 1) / BK * BK;
-    const int n_out = activation == GEMM_ACT_SWIGLU ? N / 2 : N;
-    std::vector<uint16_t> ap((size_t)M * Kp, 0), wp((size_t)N * Kp, 0);
-    for (int m = 0; m < M; ++m) std::memcpy(&ap[(size_t)m * Kp], a + (size_t)m * K, (size_t)K * 2);
-    for (int n = 0; n < N; ++n) std::memcpy(&wp[(size_t)n * Kp], b + (size_t)n * K, (size_t)K * 2);
-    b200_gemm_test_desc t{};
-    t.a = ap.data();
-    t.a_len = (int64_t)ap.size();
-    t.w = wp.data();
-    t.w_len = (int64_t)wp.size();
-    t.bias = bias;
-    t.bias_len = bias ? N : 0;
-    t.out = c;
-    t.out_len = (int64_t)M * n_out;
-    t.batches = 1;
-    t.rows_per_batch = M;
-    t.a_row_stride = Kp;
-    t.a_batch_stride = (int64_t)M * Kp;
-    t.K = Kp;
-    t.N = N;
-    t.act = activation;
-    t.out_m1 = 1;
-    t.out_s0 = n_out;
-    test_gemm_desc_host(device, t);
-}
-
-// E4M3 operands (A [M][K], W [N][K] bytes, K zero-padded to a multiple of 128): the plain epilogue with an optional deepnorm
-// residual (c = A W^T + alpha * residual, fp16) or the SwiGLU epilogue (c = E4M3 [M][N / 2]).
-void test_gemm_fp8_host(int device, const uint8_t* a, const uint8_t* b, int M, int N, int K, int activation,
-                        const uint16_t* residual, float alpha, void* c) {
-    if (M < 1 || N < 1 || K < 1) throw std::invalid_argument("test_gemm_fp8: empty operand");
-    if (activation != GEMM_ACT_NONE && activation != GEMM_ACT_SWIGLU) throw std::invalid_argument("test_gemm_fp8: plain or SwiGLU only");
-    if (residual && activation != GEMM_ACT_NONE) throw std::invalid_argument("test_gemm_fp8: the residual goes with the plain epilogue");
+    plan_gemm(d);
     require_sm90(device);
-    const int Kp = (K + BK8 - 1) / BK8 * BK8;
-    const bool swiglu = activation == GEMM_ACT_SWIGLU;
-    const int n_out = swiglu ? N / 2 : N;
-    const size_t out_bytes = (size_t)M * n_out * (swiglu ? 1 : 2);
-    uint8_t *d_a = nullptr, *d_w = nullptr;
+    const size_t ei = elem_bytes(d.in_type), eo = elem_bytes(d.out_type);
+    auto bytes = [](int64_t n, size_t elem) { return (size_t)(n > 0 ? n : 1) * elem; };
+    uint8_t *d_a = nullptr, *d_w = nullptr, *d_out = nullptr;
     __half* d_res = nullptr;
-    void* d_c = nullptr;
+    float *d_bias = nullptr, *d_gain = nullptr, *d_a_ss = nullptr, *d_res_ss = nullptr, *d_out_ss = nullptr, *d_rope = nullptr;
+    float *d_col = nullptr, *d_row = nullptr;
     Arena arena;
     arena.allocate([&](Bump& b) {
-        d_a = b.take<uint8_t>((size_t)M * Kp);
-        d_w = b.take<uint8_t>((size_t)N * Kp);
-        d_res = b.take<__half>((size_t)M * N * 2);
-        d_c = b.take(out_bytes);
+        d_a = b.take<uint8_t>(bytes(t.a_len, ei));
+        d_w = b.take<uint8_t>(bytes(t.w_len, ei));
+        d_bias = b.take<float>(bytes(t.bias_len, 4));
+        d_res = b.take<__half>(bytes(t.residual_len, 2));
+        d_gain = b.take<float>(bytes(t.res_gain_len, 4));
+        d_a_ss = b.take<float>(bytes(t.a_ss_len, 4));
+        d_res_ss = b.take<float>(bytes(t.res_ss_len, 4));
+        d_out = b.take<uint8_t>(bytes(t.out_len, eo));
+        d_out_ss = b.take<float>(bytes(t.out_ss_len, 4));
+        d_rope = b.take<float>(bytes((int64_t)rope.size(), 4));
+        d_col = b.take<float>(bytes(t.col_scale_len, 4));
+        d_row = b.take<float>(bytes(t.row_scale_len, 4));
     });
-    B200_CUDA(cudaMemset(d_a, 0, (size_t)M * Kp));
-    B200_CUDA(cudaMemset(d_w, 0, (size_t)N * Kp));
-    B200_CUDA(cudaMemcpy2D(d_a, (size_t)Kp, a, (size_t)K, (size_t)K, M, cudaMemcpyHostToDevice));
-    B200_CUDA(cudaMemcpy2D(d_w, (size_t)Kp, b, (size_t)K, (size_t)K, N, cudaMemcpyHostToDevice));
-    if (residual) B200_CUDA(cudaMemcpy(d_res, residual, (size_t)M * N * 2, cudaMemcpyHostToDevice));
-    GemmDesc d{};
-    d.fp8 = 1;
+    auto up = [](void* dst, const void* src, int64_t n, size_t elem) {
+        if (src && n > 0) B200_CUDA(cudaMemcpy(dst, src, (size_t)n * elem, cudaMemcpyHostToDevice));
+    };
+    up(d_a, t.a, t.a_len, ei);
+    up(d_w, t.w, t.w_len, ei);
+    up(d_bias, t.bias, t.bias_len, 4);
+    up(d_res, t.residual, t.residual_len, 2);
+    up(d_gain, t.res_gain, t.res_gain_len, 4);
+    up(d_a_ss, t.a_ss, t.a_ss_len, 4);
+    up(d_res_ss, t.res_ss, t.res_ss_len, 4);
+    up(d_out, t.out, t.out_len, eo);
+    up(d_rope, rope.data(), (int64_t)rope.size(), 4);
+    up(d_col, t.col_scale, t.col_scale_len, 4);
+    up(d_row, t.row_scale, t.row_scale_len, 4);
+    if (t.out_ss) B200_CUDA(cudaMemset(d_out_ss, 0xff, bytes(t.out_ss_len, 4)));   // NaN: a partial never written shows
+    // the same descriptor on the device copies
     d.a = d_a;
-    d.batches = 1;
-    d.rows_per_batch = M;
-    d.a_row_stride = Kp;
-    d.a_batch_stride = (int64_t)M * Kp;
     d.w = d_w;
-    d.N = N;
-    d.K = Kp;
-    d.act = activation;
-    d.out = d_c;
-    d.out_m1 = 1;
-    d.out_s0 = n_out;
-    d.out_s1 = 0;
-    d.residual = residual ? d_res : nullptr;
-    d.alpha = alpha;
+    d.out = d_out + t.out_offset * eo;
+    if (d.rope) d.rope = d_rope;
+    if (d.bias) d.bias = d_bias;
+    if (d.residual) d.residual = d_res;
+    if (d.res_gain) d.res_gain = d_gain;
+    if (d.a_ss) d.a_ss = d_a_ss;
+    if (d.res_ss) d.res_ss = d_res_ss;
+    if (d.out_ss) d.out_ss = d_out_ss;
+    if (d.col_scale) d.col_scale = d_col;
+    if (d.row_scale) d.row_scale = d_row;
     const GemmPlan plan = make_gemm_plan(d);
     run_gemm(plan, nullptr);
     B200_CUDA(cudaDeviceSynchronize());
-    B200_CUDA(cudaMemcpy(c, d_c, out_bytes, cudaMemcpyDeviceToHost));
-}
-
-namespace {
-
-// The int8 GEMM on host operands (A [M][K], W [N][K], K zero-padded to a multiple of 128 here) into fp16 c [M][N]: the
-// descriptor's factors, bias and RoPE table (rope: empty, or rope_table()'s positions per dim pair) as given
-void gemm_s8_host(int device, const int8_t* a, const int8_t* b, const float* row_scale, const float* col_scale,
-                  const float* bias, int M, int N, int K, int activation, const std::vector<float>& rope, int max_seq_len,
-                  int rope_T, int rope_cols, uint16_t* c) {
-    require_sm90(device);
-    const int Kp = (K + BK8 - 1) / BK8 * BK8;
-    int8_t *d_a = nullptr, *d_w = nullptr;
-    float *d_row = nullptr, *d_scale = nullptr, *d_bias = nullptr, *d_rope = nullptr;
-    __half* d_c = nullptr;
-    Arena arena;
-    arena.allocate([&](Bump& bump) {
-        d_a = bump.take<int8_t>((size_t)M * Kp);
-        d_w = bump.take<int8_t>((size_t)N * Kp);
-        d_row = bump.take<float>((size_t)M * 4);
-        d_scale = bump.take<float>((size_t)N * 4);
-        d_bias = bump.take<float>((size_t)N * 4);
-        d_rope = bump.take<float>((rope.empty() ? 1 : rope.size()) * 4);
-        d_c = bump.take<__half>((size_t)M * N * 2);
-    });
-    B200_CUDA(cudaMemset(d_a, 0, (size_t)M * Kp));
-    B200_CUDA(cudaMemset(d_w, 0, (size_t)N * Kp));
-    B200_CUDA(cudaMemcpy2D(d_a, (size_t)Kp, a, (size_t)K, (size_t)K, M, cudaMemcpyHostToDevice));
-    B200_CUDA(cudaMemcpy2D(d_w, (size_t)Kp, b, (size_t)K, (size_t)K, N, cudaMemcpyHostToDevice));
-    if (row_scale) B200_CUDA(cudaMemcpy(d_row, row_scale, (size_t)M * 4, cudaMemcpyHostToDevice));
-    B200_CUDA(cudaMemcpy(d_scale, col_scale, (size_t)N * 4, cudaMemcpyHostToDevice));
-    if (bias) B200_CUDA(cudaMemcpy(d_bias, bias, (size_t)N * 4, cudaMemcpyHostToDevice));
-    if (!rope.empty()) B200_CUDA(cudaMemcpy(d_rope, rope.data(), rope.size() * 4, cudaMemcpyHostToDevice));
-    GemmDesc d{};
-    d.q8 = GEMM_Q8_OPERANDS;
-    d.col_scale = d_scale;
-    d.row_scale = row_scale ? d_row : nullptr;
-    d.a = d_a;
-    d.batches = 1;
-    d.rows_per_batch = M;
-    d.a_row_stride = Kp;
-    d.a_batch_stride = (int64_t)M * Kp;
-    d.w = d_w;
-    d.N = N;
-    d.K = Kp;
-    d.bias = bias ? d_bias : nullptr;
-    d.act = activation;
-    d.out = d_c;
-    d.out_m1 = 1;
-    d.out_s0 = N;
-    d.out_s1 = 0;
-    if (!rope.empty()) {
-        d.rope = d_rope;
-        d.rope_T = rope_T;
-        d.rope_cols = rope_cols;
-        d.rope_stride = max_seq_len;
-    }
-    const GemmPlan plan = make_gemm_plan(d);
-    run_gemm(plan, nullptr);
-    B200_CUDA(cudaDeviceSynchronize());
-    B200_CUDA(cudaMemcpy(c, d_c, (size_t)M * N * 2, cudaMemcpyDeviceToHost));
-}
-
-}  // namespace
-
-// int8 operands (A [M][K], W [N][K], K zero-padded to a multiple of 128): c = act(float(A W^T) * col_scale[n] + bias[n]), fp16
-void test_gemm_s8_host(int device, const int8_t* a, const int8_t* b, const float* col_scale, const float* bias, int M, int N,
-                       int K, int activation, uint16_t* c) {
-    if (M < 1 || N < 1 || K < 1) throw std::invalid_argument("test_gemm_s8: empty operand");
-    gemm_s8_host(device, a, b, nullptr, col_scale, bias, M, N, K, activation, {}, 0, 0, 0, c);
-}
-
-// int8 operands with per-row and per-column factors: v = (float(A W^T) * row_scale[m]) * col_scale[n]; c = fp16(v), or with
-// GEMM_ACT_ROPE the rotary embedding of v at position m % rope_T on the first rope_cols columns (the table of
-// rope_table(theta, max_seq_len)), as the transformer's QKV projection.
-void test_gemm_s8_scaled_host(int device, const int8_t* a, const int8_t* b, const float* row_scale, const float* col_scale,
-                              int M, int N, int K, int activation, float theta, int max_seq_len, int rope_T, int rope_cols,
-                              uint16_t* c) {
-    if (M < 1 || N < 1 || K < 1 || N % 32 != 0) throw std::invalid_argument("test_gemm_s8_scaled: empty operand or N not a multiple of 32");
-    if (activation != GEMM_ACT_NONE && activation != GEMM_ACT_ROPE) throw std::invalid_argument("test_gemm_s8_scaled: plain or RoPE only");
-    const bool rope = activation == GEMM_ACT_ROPE;
-    if (rope && !(theta > 0.0f && max_seq_len >= 1 && max_seq_len <= (1 << 16) && rope_T >= 1 && rope_T <= max_seq_len &&
-                  rope_cols >= 0 && rope_cols <= N && rope_cols % 64 == 0 && N % 64 == 0)) {
-        throw std::invalid_argument("test_gemm_s8_scaled: RoPE needs theta > 0, 1 <= rope_T <= max_seq_len and whole 64-column heads");
-    }
-    gemm_s8_host(device, a, b, row_scale, col_scale, nullptr, M, N, K, activation,
-                 rope ? rope_table(theta, max_seq_len) : std::vector<float>(), max_seq_len, rope_T, rope_cols, c);
+    B200_CUDA(cudaMemcpy(t.out, d_out, (size_t)t.out_len * eo, cudaMemcpyDeviceToHost));
+    if (t.out_ss) B200_CUDA(cudaMemcpy(t.out_ss, d_out_ss, (size_t)rows * (t.N / 32) * 4, cudaMemcpyDeviceToHost));
 }
 
 }  // namespace b200

@@ -1,6 +1,6 @@
-// wgmma GEMM with fused epilogue:  out[row(g)][n] = act( sum_k A[g][k] * W[n][k] + bias[n] ), fp16 in/out (or E4M3
-// operands, GemmDesc::fp8), fp32 accumulation in registers; or int8 operands with exact s32 accumulation and a per-column
-// dequantisation factor (GemmDesc::q8).  See gemm.cu.
+// wgmma GEMM with fused epilogue:  out[row(g)][n] = act( sum_k A[g][k] * W[n][k] + bias[n] ), fp32 accumulation in
+// registers (exact s32 for int8 operands).  GemmDesc::in_type and out_type name the element types; gemm.cu's table of kernel
+// forms lists the combinations that run.
 #pragma once
 
 #include "tc.cuh"
@@ -17,45 +17,45 @@ enum GemmAct : int {
     GEMM_ACT_ROPE = 5,         // output columns are [3][H][64] (q|k|v): rotary embedding on q and k (TxModules.cpp:220-250)
 };
 
-// The int8 precision of the LSTM models (GemmDesc::q8)
-enum GemmQ8 : int {
-    GEMM_Q8_NONE = 0,
-    GEMM_Q8_OPERANDS = 1,  // A and W are int8: exact s32 accumulation, out = act(float(acc) * col_scale[n] + bias[n]) as fp16
-                           // (float(acc) * row_scale[g] first when GemmDesc::row_scale is set)
-    GEMM_Q8_STORE = 2,     // fp16 operands, GEMM_ACT_TANH: the output is int8 cvt.rni.sat(kInt8ActScale * tanh(v))
+// Element type of the GEMM's operands (A and W) or of its output
+enum GemmType : int {
+    GEMM_F16 = 0,
+    GEMM_E4M3 = 1,
+    GEMM_S8 = 2,
 };
 // int8 value of an activation v in [-1, 1] (the last convolution's tanh output and every h_t of an int8 LSTM layer).  The
 // reference's factor is inside closed Koi; 127 is this engine's choice: the symmetric range, so -128 never appears.
 constexpr float kInt8ActScale = 127.0f;
 
 struct GemmDesc {
-    // fp8 = 1: A and W are E4M3 bytes (K a multiple of 128, one 128-byte TMA box row per K block), and the SwiGLU epilogue
-    // writes E4M3; every other epilogue writes fp16.  Only GEMM_ACT_NONE and GEMM_ACT_SWIGLU have E4M3 forms.
-    int fp8 = 0;
-    // q8: GemmQ8.  GEMM_Q8_OPERANDS takes int8 bytes with the E4M3 form's addressing (K a multiple of 128), the plain and
-    // TANH_X5 activations, a column bias and col_scale [N] (fp32 dequantisation factor per output column).
-    // GEMM_Q8_STORE writes int8 where the fp16 form writes fp16: out is int8 and its strides count bytes.
-    // row_scale [batches * rows_per_batch] (optional, GEMM_Q8_OPERANDS only): fp32 dequantisation factor per A row, applied
-    // as v = (float(acc) * row_scale[g]) * col_scale[n], each product rounded in fp32.  With it the form also takes
-    // GEMM_ACT_ROPE (no bias), whose rotation then runs on v (the int8_qkv_fp8_ffn transformer's QKV projection).
-    int q8 = GEMM_Q8_NONE;
+    // in_type: A and W.  E4M3 and int8 take one byte per element, so a K block (one 128-byte TMA box row) is 128 elements
+    // instead of 64 and K must be a multiple of 128.  int8 operands accumulate exactly in s32 and need col_scale [N], the
+    // fp32 dequantisation factor per output column: v = float(acc) * col_scale[n] + bias[n].  With row_scale
+    // [batches * rows_per_batch], the fp32 factor per A row, they take their own kernel forms:
+    // v = (float(acc) * row_scale[g]) * col_scale[n] (+ bias[n]), each product rounded in fp32.
+    // out_type: the stored element; out's strides count elements of it.  E4M3 goes with E4M3 operands and SwiGLU; int8 with
+    // fp16 operands and tanh, stored as cvt.rni.sat(kInt8ActScale * tanh(v)).
+    // gemm.cu's table lists the (in_type, out_type, act, row_scale set) forms and the optional inputs each one reads;
+    // make_gemm_plan refuses any other combination, and any optional input the form does not read.
+    GemmType in_type = GEMM_F16;
+    GemmType out_type = GEMM_F16;
     const float* col_scale = nullptr;
     const float* row_scale = nullptr;
-    // A: logical [batches][rows_per_batch][K] fp16, K contiguous; row/batch strides in elements
+    // A: logical [batches][rows_per_batch][K] of in_type, K contiguous; row/batch strides in elements
     const void* a = nullptr;
     int batches = 1;
     int rows_per_batch = 0;
     int64_t a_row_stride = 0;
     int64_t a_batch_stride = 0;
-    // W: [N][K] fp16 (K contiguous, row stride = K_pad)
+    // W: [N][K] of in_type (K contiguous, row stride = K_pad)
     const void* w = nullptr;
     int N = 0;
-    int K = 0;  // multiple of 64 (128 for fp8; pad weights with zeros)
+    int K = 0;  // multiple of 64 (128 for E4M3 and int8; pad weights with zeros)
     int a_inner = 0;  // extent of A's K dimension in the tensor map (0 = K); elements beyond read as zero
     const float* bias = nullptr;
     int act = GEMM_ACT_NONE;
     // output: global row g = batch * rows_per_batch + row  ->  out + (g / out_m1) * out_s0 + (g % out_m1) * out_s1
-    void* out = nullptr;   // fp16, or E4M3 bytes (fp8 SwiGLU)
+    void* out = nullptr;   // out_type
     int64_t out_m1 = 1;
     int64_t out_s0 = 0;
     int64_t out_s1 = 0;
@@ -88,6 +88,8 @@ struct GemmDesc {
 struct GemmPlan {
     CUtensorMap tma_a, tma_w;
     GemmDesc d;
+    const void* kernel = nullptr;   // the descriptor's gemm_wgmma_kernel form
+    int num_k_blocks = 0;
     int bn = 128;
     int tiles_per_batch = 0;
     dim3 grid;

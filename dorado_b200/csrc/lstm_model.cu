@@ -1200,7 +1200,7 @@ LstmStack::LstmStack(const LstmStackDesc& d, const LstmStackBuffers& ws) : m_d(d
         g.N = 4 * C;
         g.K = (C + 63) / 64 * 64;
         if (d.int8) {   // rows of int8, K = C = whole 128-byte blocks
-            g.q8 = GEMM_Q8_OPERANDS;
+            g.in_type = GEMM_S8;
             g.w = w.w_ih8;
             g.col_scale = w.inv;
             g.K = C;
@@ -1553,7 +1553,7 @@ std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half*
         g.K = K3p;
         g.bias = b3;
         g.act = desc.convs[2].activation;
-        g.q8 = int8 ? GEMM_Q8_STORE : GEMM_Q8_NONE;
+        g.out_type = int8 ? GEMM_S8 : GEMM_F16;
         g.out = seq;
         g.out_m1 = T_out;        // g = n * T_out + t
         g.out_s0 = C;            // n
@@ -1587,7 +1587,7 @@ std::unique_ptr<ForwardPlan> LstmModel::make_plan(int N, int T_in, const __half*
         g.a_inner = C;
         g.bias = bl1;
         if (int8) {
-            g.q8 = GEMM_Q8_OPERANDS;
+            g.in_type = GEMM_S8;
             g.w = wl1_8;
             g.col_scale = wl1_inv;
             g.K = C;

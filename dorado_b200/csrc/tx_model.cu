@@ -790,16 +790,17 @@ std::unique_ptr<ForwardPlan> TxModel::make_plan(int N, int T_in, const __half* s
             // with RoPE; out_proj -> y (+ alpha * x); norm1 y -> att (fp16) + qkv's buffer (E4M3); fc1 + SwiGLU -> hid
             // (E4M3); fc2 -> y (+ alpha * att); norm2 y -> x (fp16) + x8 / x_inv
             GemmDesc q = dense(x8, dm, lw.wqkv_i8, dqkv, nullptr, GEMM_ACT_ROPE, qkv, dqkv, nullptr, 0.0f);
-            q.q8 = GEMM_Q8_OPERANDS;
+            q.in_type = GEMM_S8;
             q.row_scale = x_inv;
             q.col_scale = lw.wqkv_inv;
             L.qkv = make_gemm_plan(q);
             L.out_proj = make_gemm_plan(dense(att, dm, lw.wo, dm, lw.bo, GEMM_ACT_NONE, y, dm, x, desc.deepnorm_alpha));
             GemmDesc f1 = dense(qkv, dm, lw.w1_e4m3, 2 * ff, nullptr, GEMM_ACT_SWIGLU, hid, ff, nullptr, 0.0f);
-            f1.fp8 = 1;
+            f1.in_type = GEMM_E4M3;
+            f1.out_type = GEMM_E4M3;
             L.fc1 = make_gemm_plan(f1);
             GemmDesc f2 = dense(hid, ff, lw.w2_e4m3, dm, nullptr, GEMM_ACT_NONE, y, dm, att, desc.deepnorm_alpha);
-            f2.fp8 = 1;
+            f2.in_type = GEMM_E4M3;
             L.fc2 = make_gemm_plan(f2);
         } else if (fp8) {
             // qkv and out_proj as in the folded fp16 layout; norm1 -> att (fp16) + qkv's buffer (E4M3, free once attention has
@@ -812,10 +813,11 @@ std::unique_ptr<ForwardPlan> TxModel::make_plan(int N, int T_in, const __half* s
             if (!first) { o.res_ss = ss_a; o.res_ss_parts = ssp; o.res_gain = layers[l - 1].n2; }
             L.out_proj = make_gemm_plan(o);
             GemmDesc f1 = dense(qkv, dm, lw.w1_e4m3, 2 * ff, nullptr, GEMM_ACT_SWIGLU, hid, ff, nullptr, 0.0f);
-            f1.fp8 = 1;
+            f1.in_type = GEMM_E4M3;
+            f1.out_type = GEMM_E4M3;
             L.fc1 = make_gemm_plan(f1);
             GemmDesc f2 = dense(hid, ff, lw.w2_e4m3, dm, nullptr, GEMM_ACT_NONE, x, dm, att, desc.deepnorm_alpha);
-            f2.fp8 = 1;
+            f2.in_type = GEMM_E4M3;
             f2.out_ss = ss_a;
             L.fc2 = make_gemm_plan(f2);
         } else if (fold_norm) {

@@ -98,7 +98,14 @@ class GemmTestDesc(C.Structure):
         ("alpha", C.c_float), ("a_ss_parts", C.c_int32), ("res_ss_parts", C.c_int32), ("norm_dim", C.c_int32),
         ("norm_eps", C.c_float), ("max_ctas", C.c_int32), ("theta", C.c_float),
         ("max_seq_len", C.c_int32), ("rope_T", C.c_int32), ("rope_cols", C.c_int32),
+        ("in_type", C.c_int32), ("out_type", C.c_int32), ("col_scale", C.c_void_p), ("col_scale_len", C.c_int64),
+        ("row_scale", C.c_void_p), ("row_scale_len", C.c_int64),
     ]
+
+
+# GemmType (dorado_b200/csrc/gemm.h): the element types of b200_gemm_test_desc's in_type and out_type, and their numpy types
+GEMM_F16, GEMM_E4M3, GEMM_S8 = 0, 1, 2
+GEMM_DTYPES = {GEMM_F16: np.float16, GEMM_E4M3: np.uint8, GEMM_S8: np.int8}
 
 
 class Stats(C.Structure):
@@ -112,7 +119,7 @@ EXPORTS = [
     "b200_runner_set_decoder_options", "b200_runner_batch_size", "b200_runner_chunk_size", "b200_runner_out_len",
     "b200_runner_accept_chunk_f16", "b200_runner_accept_chunk_f32", "b200_runner_input", "b200_runner_call_chunks",
     "b200_runner_upload", "b200_runner_step_device", "b200_runners_step_device", "b200_runner_forward_scores", "b200_runner_profile", "b200_runner_plan_info", "b200_runner_debug_read_workspace", "b200_decode_scores",
-    "b200_test_gemm", "b200_test_gemm_desc", "b200_test_gemm_fp8", "b200_test_gemm_s8", "b200_test_gemm_s8_scaled", "b200_test_quantize_act_rows", "b200_test_quantize_rows", "b200_test_to_e4m3", "b200_test_remove_bits", "b200_test_attention", "b200_generate_chunks", "b200_stitch_chunks", "b200_runner_accept_raw_chunk",
+    "b200_test_gemm_desc", "b200_test_quantize_act_rows", "b200_test_quantize_rows", "b200_test_to_e4m3", "b200_test_remove_bits", "b200_test_attention", "b200_generate_chunks", "b200_stitch_chunks", "b200_runner_accept_raw_chunk",
     "b200_runner_debug_read_input", "b200_engine_runner_bytes", "b200_engine_benchmark_batch_sizes",
     "b200_select_batch_size", "b200_generate_variable_chunks", "b200_engine_terminate", "b200_engine_restart",
     "b200_engine_set_low_latency", "b200_engine_is_low_latency", "b200_engine_batch_timeouts_ms",
@@ -195,13 +202,9 @@ def load_library() -> C.CDLL:
     lib.b200_runner_profile.argtypes = [vp, i32, C.c_char_p, C.c_uint64]
     lib.b200_runner_plan_info.argtypes = [vp, C.c_char_p, C.c_uint64]
     lib.b200_runner_debug_read_workspace.argtypes = [vp, C.c_uint64, C.c_uint64, vp]
-    lib.b200_test_gemm.argtypes = [i32, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.b200_test_gemm_desc.argtypes = [i32, C.POINTER(GemmTestDesc)]
     lib.b200_test_attention.argtypes = [i32, vp, i32, i32, i32, i32, i32, vp]
-    lib.b200_test_gemm_fp8.argtypes = [i32, vp, vp, i32, i32, i32, i32, vp, f32, vp]
-    lib.b200_test_gemm_s8.argtypes = [i32, vp, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.b200_test_quantize_rows.argtypes = [vp, i32, i32, vp, vp]
-    lib.b200_test_gemm_s8_scaled.argtypes = [i32, vp, vp, vp, vp, i32, i32, i32, i32, f32, i32, i32, i32, vp]
     lib.b200_test_quantize_act_rows.argtypes = [i32, vp, i32, i32, vp, vp]
     lib.b200_test_to_e4m3.argtypes = [vp, C.c_int64, vp]
     lib.b200_test_remove_bits.argtypes = [vp, C.c_int64, i32, vp]
@@ -299,40 +302,27 @@ def decode_scores(scores: np.ndarray, clamp_val: float = 0.0, opts: DecoderOptio
     return moves, seq, qstr, nb
 
 
-def test_gemm(a: np.ndarray, b: np.ndarray, bias: np.ndarray | None, activation: int = -1, device: int = 0):
-    lib = load_library()
-    a = np.ascontiguousarray(a, np.float16)
-    b = np.ascontiguousarray(b, np.float16)
-    M, K = a.shape
-    N = b.shape[0]
-    c = np.empty((M, N // 2 if activation == 4 else N), np.float16)
-    bias_p = None
-    if bias is not None:
-        bias = np.ascontiguousarray(bias, np.float32)
-        bias_p = bias.ctypes.data
-    check(lib.b200_test_gemm(device, a.ctypes.data, b.ctypes.data, bias_p, M, N, K, activation, c.ctypes.data))
-    return c
-
-
 def test_gemm_desc(a: np.ndarray, w: np.ndarray, out: np.ndarray, *, rows_per_batch: int, a_row_stride: int, out_s0: int,
                    batches: int = 1, a_batch_stride: int = 0, a_inner: int = 0, act: int = -1, out_offset: int = 0,
                    out_m1: int = 1, out_s1: int = 0, bias=None, residual=None, alpha: float = 0.0, res_gain=None,
                    a_ss=None, a_ss_parts: int = 0, res_ss=None, res_ss_parts: int = 0, norm_dim: int = 0,
                    norm_eps: float = 1e-5, max_ctas: int = 0, theta: float = 0.0, max_seq_len: int = 0, rope_T: int = 0,
-                   rope_cols: int = 0, out_ss: bool = False, device: int = 0):
-    """The fp16 GEMM launched from a full descriptor (b200_test_gemm_desc): a is any flat fp16 buffer, w [N, K] fp16, out the
-    whole output buffer with the caller's sentinel in it.  Returns (the output buffer after the GEMM, the [rows, N / 32]
-    partial sums of squares or None)."""
+                   rope_cols: int = 0, out_ss: bool = False, in_type: int = GEMM_F16, out_type: int = GEMM_F16,
+                   col_scale=None, row_scale=None, device: int = 0):
+    """The GEMM launched from a full descriptor (b200_test_gemm_desc): a is any flat buffer and w [N, K] of in_type, out the
+    whole output buffer of out_type with the caller's sentinel in it (GEMM_DTYPES gives the numpy types).  Returns (the
+    output buffer after the GEMM, the [rows, N / 32] partial sums of squares or None)."""
     lib = load_library()
     flat = lambda x, t: None if x is None else np.ascontiguousarray(np.ravel(x), t)
-    a, res, outb = flat(a, np.float16), flat(residual, np.float16), flat(out, np.float16).copy()
-    w = np.ascontiguousarray(w, np.float16)
-    bias, res_gain, a_ss, res_ss = (flat(x, np.float32) for x in (bias, res_gain, a_ss, res_ss))
+    a, res, outb = flat(a, GEMM_DTYPES[in_type]), flat(residual, np.float16), flat(out, GEMM_DTYPES[out_type]).copy()
+    w = np.ascontiguousarray(w, GEMM_DTYPES[in_type])
+    bias, res_gain, a_ss, res_ss, col_scale, row_scale = (flat(x, np.float32) for x in (bias, res_gain, a_ss, res_ss,
+                                                                                         col_scale, row_scale))
     N, K = w.shape
     ss = np.empty((batches * rows_per_batch, N // 32), np.float32) if out_ss else None
     d = GemmTestDesc()
     for name, arr in (("a", a), ("w", w), ("bias", bias), ("residual", res), ("res_gain", res_gain), ("a_ss", a_ss),
-                      ("res_ss", res_ss), ("out", outb), ("out_ss", ss)):
+                      ("res_ss", res_ss), ("out", outb), ("out_ss", ss), ("col_scale", col_scale), ("row_scale", row_scale)):
         if arr is not None:
             setattr(d, name, arr.ctypes.data)
             setattr(d, name + "_len", arr.size)
@@ -341,66 +331,61 @@ def test_gemm_desc(a: np.ndarray, w: np.ndarray, out: np.ndarray, *, rows_per_ba
     d.out_offset, d.out_m1, d.out_s0, d.out_s1 = out_offset, out_m1, out_s0, out_s1
     d.alpha, d.a_ss_parts, d.res_ss_parts, d.norm_dim, d.norm_eps = alpha, a_ss_parts, res_ss_parts, norm_dim, norm_eps
     d.max_ctas, d.theta, d.max_seq_len, d.rope_T, d.rope_cols = max_ctas, theta, max_seq_len, rope_T, rope_cols
+    d.in_type, d.out_type = in_type, out_type
     check(lib.b200_test_gemm_desc(device, C.byref(d)))
     return outb, ss
+
+
+def _test_gemm_dense(a, b, activation, in_type, out_type=GEMM_F16, device=0, **inputs):
+    """test_gemm_desc on dense operands a [M, K] and b [N, K] of in_type, K zero-padded to a whole K block (64 fp16 or
+    128 one-byte elements): out_type [M, N] (N / 2 with SwiGLU)."""
+    a = np.ascontiguousarray(a, GEMM_DTYPES[in_type])
+    b = np.ascontiguousarray(b, GEMM_DTYPES[in_type])
+    (M, K), N = a.shape, b.shape[0]
+    kb = 64 if in_type == GEMM_F16 else 128
+    Kp = (K + kb - 1) // kb * kb
+    pad = lambda x: np.pad(x, ((0, 0), (0, Kp - K)))
+    n_out = N // 2 if activation == 4 else N
+    out = np.zeros(M * n_out, GEMM_DTYPES[out_type])
+    c, _ = test_gemm_desc(pad(a), pad(b), out, rows_per_batch=M, a_row_stride=Kp, out_s0=n_out, act=activation,
+                          in_type=in_type, out_type=out_type, device=device, **inputs)
+    return c.reshape(M, n_out)
+
+
+def test_gemm(a: np.ndarray, b: np.ndarray, bias: np.ndarray | None, activation: int = -1, device: int = 0):
+    """The fp16 GEMM on host data: a [M, K], b [N, K] fp16 -> fp16 [M, N] (N / 2 with SwiGLU) of act(a b^T + bias)."""
+    return _test_gemm_dense(a, b, activation, GEMM_F16, bias=bias, device=device)
 
 
 def test_gemm_fp8(a: np.ndarray, b: np.ndarray, activation: int = -1, residual: np.ndarray | None = None,
                   alpha: float = 0.0, device: int = 0):
     """The E4M3 GEMM on host data: a [M, K], b [N, K] E4M3 bytes (uint8) -> fp16 [M, N] (activation -1, optionally
     + alpha * residual [M, N] fp16) or E4M3 bytes [M, N / 2] (activation 4, SwiGLU)."""
-    lib = load_library()
-    a = np.ascontiguousarray(a, np.uint8)
-    b = np.ascontiguousarray(b, np.uint8)
-    M, K = a.shape
-    N = b.shape[0]
-    c = np.empty((M, N // 2), np.uint8) if activation == 4 else np.empty((M, N), np.float16)
-    res_p = None
     if residual is not None:
         residual = np.ascontiguousarray(residual, np.float16)
-        assert residual.shape == (M, N)
-        res_p = residual.ctypes.data
-    check(lib.b200_test_gemm_fp8(device, a.ctypes.data, b.ctypes.data, M, N, K, activation, res_p, alpha, c.ctypes.data))
-    return c
+        assert residual.shape == (np.shape(a)[0], np.shape(b)[0])
+    return _test_gemm_dense(a, b, activation, GEMM_E4M3, GEMM_E4M3 if activation == 4 else GEMM_F16, residual=residual,
+                            alpha=alpha, device=device)
 
 
 def test_gemm_s8(a: np.ndarray, b: np.ndarray, col_scale: np.ndarray, bias: np.ndarray | None = None, activation: int = -1,
                  device: int = 0):
     """The int8 GEMM on host data: a [M, K], b [N, K] int8 -> fp16 [M, N] of act(float(a b^T) * col_scale + bias)."""
-    lib = load_library()
-    a = np.ascontiguousarray(a, np.int8)
-    b = np.ascontiguousarray(b, np.int8)
-    M, K = a.shape
-    N = b.shape[0]
     col_scale = np.ascontiguousarray(col_scale, np.float32)
-    assert col_scale.shape == (N,)
-    bias_p = None
-    if bias is not None:
-        bias = np.ascontiguousarray(bias, np.float32)
-        bias_p = bias.ctypes.data
-    c = np.empty((M, N), np.float16)
-    check(lib.b200_test_gemm_s8(device, a.ctypes.data, b.ctypes.data, col_scale.ctypes.data, bias_p, M, N, K, activation,
-                                c.ctypes.data))
-    return c
+    assert col_scale.shape == (np.shape(b)[0],)
+    return _test_gemm_dense(a, b, activation, GEMM_S8, col_scale=col_scale, bias=bias, device=device)
 
 
 def test_gemm_s8_scaled(a: np.ndarray, b: np.ndarray, row_scale: np.ndarray, col_scale: np.ndarray, activation: int = -1,
-                       theta: float = 0.0, max_seq_len: int = 0, rope_T: int = 0, rope_cols: int = 0, device: int = 0):
+                        theta: float = 0.0, max_seq_len: int = 0, rope_T: int = 0, rope_cols: int = 0, device: int = 0):
     """The int8 GEMM with per-row and per-column factors on host data: a [M, K], b [N, K] int8 -> fp16 [M, N] of
     (float(a b^T) * row_scale[m]) * col_scale[n], with RoPE at position m % rope_T on the first rope_cols columns when
-    activation is 5 (b200_test_gemm_s8_scaled)."""
-    lib = load_library()
-    a = np.ascontiguousarray(a, np.int8)
-    b = np.ascontiguousarray(b, np.int8)
-    M, K = a.shape
-    N = b.shape[0]
+    activation is 5."""
     row_scale = np.ascontiguousarray(row_scale, np.float32)
     col_scale = np.ascontiguousarray(col_scale, np.float32)
-    assert row_scale.shape == (M,) and col_scale.shape == (N,)
-    c = np.empty((M, N), np.float16)
-    check(lib.b200_test_gemm_s8_scaled(device, a.ctypes.data, b.ctypes.data, row_scale.ctypes.data, col_scale.ctypes.data, M, N,
-                                       K, activation, theta, max_seq_len, rope_T, rope_cols, c.ctypes.data))
-    return c
+    assert row_scale.shape == (np.shape(a)[0],) and col_scale.shape == (np.shape(b)[0],)
+    return _test_gemm_dense(a, b, activation, GEMM_S8, row_scale=row_scale, col_scale=col_scale, theta=theta,
+                            max_seq_len=max_seq_len, rope_T=rope_T, rope_cols=rope_cols, device=device)
 
 
 def quantize_act_rows(x: np.ndarray, device: int = 0):

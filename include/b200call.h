@@ -510,24 +510,6 @@ B200_API int b200_modbase_runner_profile(b200_modbase_runner* runner, char* buf,
 B200_API int b200_modbase_runner_debug_read_workspace(b200_modbase_runner* runner, uint64_t offset, uint64_t bytes, void* dst);
 
 /* Kernel-level test hooks (host buffers; used by tests/ only). */
-/* The GEMM with E4M3 operands (A [M,K], W [N,K] bytes; K is zero-padded to a multiple of 128 inside).  activation -1:
- * c = A W^T (+ alpha * residual when residual [M,N] fp16 is given), fp16 [M,N].  activation 4 (SwiGLU, columns (2i, 2i+1)
- * = (y, gate)): c = E4M3 [M,N/2] of y * silu(gate). */
-B200_API int b200_test_gemm_fp8(int32_t device, const uint8_t* a, const uint8_t* b, int32_t M, int32_t N, int32_t K,
-                                int32_t activation, const uint16_t* residual, float alpha, void* c);
-/* The GEMM with int8 operands (A [M,K], W [N,K]; K is zero-padded to a multiple of 128 inside):
- * c = act(float(A W^T) * col_scale[n] + bias[n]) as fp16 [M,N]; the s32 accumulation is exact.  activation -1 or 3 (tanh x 5);
- * bias may be NULL. */
-B200_API int b200_test_gemm_s8(int32_t device, const int8_t* a, const int8_t* b, const float* col_scale, const float* bias,
-                               int32_t M, int32_t N, int32_t K, int32_t activation, uint16_t* c);
-/* The GEMM with int8 operands and per-row and per-column factors (A [M,K], W [N,K]; K is zero-padded to a multiple of 128
- * inside; N a multiple of 32): v = (float(A W^T) * row_scale[m]) * col_scale[n], each product rounded in fp32, the s32 -> fp32
- * conversion to nearest even.  activation -1: c = fp16(v) [M,N].  activation 5 (RoPE, the int8_qkv_fp8_ffn QKV projection):
- * the first rope_cols columns (whole 64-column heads) rotated at position m % rope_T with the model's fp32 table for theta
- * and max_seq_len positions (1 <= rope_T <= max_seq_len), then fp16; the theta and rope arguments are ignored otherwise. */
-B200_API int b200_test_gemm_s8_scaled(int32_t device, const int8_t* a, const int8_t* b, const float* row_scale,
-                                      const float* col_scale, int32_t M, int32_t N, int32_t K, int32_t activation, float theta,
-                                      int32_t max_seq_len, int32_t rope_T, int32_t rope_cols, uint16_t* c);
 /* The int8_qkv_fp8_ffn precision's device quantiser on fp16 rows [rows, cols] (cols a positive multiple of 128): int8 q
  * [rows, cols] and fp32 inv [rows] = 1 / float(fp16(128 / absmax)), bit for bit b200_test_quantize_rows' q and the reciprocal
  * of its scale (0 where the scale is +inf). */
@@ -540,26 +522,25 @@ B200_API int b200_test_quantize_rows(const uint16_t* f16, int32_t rows, int32_t 
  * nearest even; NaN beyond the range).  remove_bits: the reference's (bits + 2^(b-1)) & ~(2^b - 1) on the int16 view. */
 B200_API int b200_test_to_e4m3(const uint16_t* f16, int64_t n, uint8_t* out);
 B200_API int b200_test_remove_bits(const uint16_t* f16, int64_t n, int32_t bits, uint16_t* out);
-B200_API int b200_test_gemm(int32_t device, const uint16_t* a /* [M,K] fp16 */, const uint16_t* b /* [N,K] fp16 */,
-                            const float* bias /* [N] or NULL */, int32_t M, int32_t N, int32_t K, int32_t activation,
-                            uint16_t* c /* [M,N] fp16 */);
-/* The fp16 GEMM launched from every field the model plans set (dorado_b200/csrc/gemm.h, GemmDesc), on host buffers.  Each
- * buffer comes with its length in elements; a descriptor that would read or write beyond one returns B200_ERR_INVALID
- * before anything is allocated.  Rows g = batch * rows_per_batch + r, r < rows_per_batch, read A at
+/* The GEMM launched from every field the model plans set (dorado_b200/csrc/gemm.h, GemmDesc), on host buffers.  in_type
+ * (A and W) and out_type are 0 fp16, 1 E4M3 or 2 int8 (GemmType); zero fields mean fp16.  Each buffer comes with its
+ * length in elements of its type; a descriptor that would read or write beyond one, or that has no kernel form or sets an
+ * input its form does not read (GemmDesc), returns B200_ERR_INVALID before anything is allocated.  Output offsets and
+ * strides count elements of out_type.  Rows g = batch * rows_per_batch + r, r < rows_per_batch, read A at
  * batch * a_batch_stride + r * a_row_stride + k for k < (a_inner ? a_inner : K) (zeros beyond, up to K) and write
  * out + out_offset + (g / out_m1) * out_s0 + (g % out_m1) * out_s1 + n for n < N (N / 2 with SwiGLU).  The residual is
  * read at g * N + n, the partial sums of squares at g * parts + i.  out holds the caller's sentinel on entry and the
  * whole buffer on return.  out_ss, when not NULL, receives the N / 32 partials of every row (NaN where none was written).
  * act 5 (RoPE) takes the model's own table for theta and max_seq_len, and rotates position g % rope_T. */
 typedef struct b200_gemm_test_desc {
-    const uint16_t* a;         int64_t a_len;         /* fp16, flat: overlapping and padded views are the caller's */
-    const uint16_t* w;         int64_t w_len;         /* fp16 [N][K] */
+    const void* a;             int64_t a_len;         /* in_type, flat: overlapping and padded views are the caller's */
+    const void* w;             int64_t w_len;         /* in_type [N][K] */
     const float* bias;         int64_t bias_len;      /* [N] or NULL */
     const uint16_t* residual;  int64_t residual_len;  /* fp16 or NULL */
     const float* res_gain;     int64_t res_gain_len;  /* [N] or NULL */
     const float* a_ss;         int64_t a_ss_len;      /* [rows][a_ss_parts] or NULL */
     const float* res_ss;       int64_t res_ss_len;    /* [rows][res_ss_parts] or NULL */
-    uint16_t* out;             int64_t out_len;       /* fp16 */
+    void* out;                 int64_t out_len;       /* out_type */
     float* out_ss;             int64_t out_ss_len;    /* [rows][N / 32] or NULL */
     int32_t batches, rows_per_batch;
     int64_t a_row_stride, a_batch_stride;
@@ -571,6 +552,9 @@ typedef struct b200_gemm_test_desc {
     int32_t max_ctas;
     float theta;
     int32_t max_seq_len, rope_T, rope_cols;
+    int32_t in_type, out_type;
+    const float* col_scale;    int64_t col_scale_len; /* [N] or NULL: required with int8 operands */
+    const float* row_scale;    int64_t row_scale_len; /* [rows] or NULL: int8 operands with per-row factors */
 } b200_gemm_test_desc;
 B200_API int b200_test_gemm_desc(int32_t device, const b200_gemm_test_desc* desc);
 /* The transformer's sliding-window attention kernel, launched exactly as the model launches it: qkv of N chunks of T tokens

@@ -2,8 +2,10 @@
 tests/test_gemm_plans_gpu.py fails for a kernel that made one of the mistakes those checks exist for (each simulated
 on the GPU test's own inputs by writing a mis-computed reference, rounded to fp16, into the sentinel buffer), while
 the correctly rounded reference passes; b200_test_gemm_desc's refusal of a descriptor that reaches beyond any buffer it
-is given, which happens before any device work; and the d_model 128 configuration the GPU test runs."""
+is given, or that has no kernel form or sets an input its form does not read, which happens before any device work; and
+the d_model 128 configuration the GPU test runs."""
 import dataclasses
+import itertools
 
 import numpy as np
 import pytest
@@ -146,17 +148,27 @@ def _hook_case():
     out_len = 4 + 300 + 2 * 128 + N
     bufs = dict(a=np.ones(a_len, np.float16), w=np.ones((N, K), np.float16), bias=np.zeros(N, np.float32),
                 residual=np.zeros(rows * N, np.float16), res_gain=np.ones(N, np.float32), a_ss=np.ones(rows * 2, np.float32),
-                res_ss=np.ones(rows * 4, np.float32), out=np.zeros(out_len, np.float16))
+                res_ss=np.ones(rows * 4, np.float32), out=np.zeros(out_len, np.float16), out_ss=np.zeros(rows * 4, np.float32))
+    return d, bufs
+
+
+def _hook_case_s8():
+    """The int8 QKV-like descriptor without RoPE: int8 operands with row and column factors and a bias, over two batches."""
+    rows, K, N = 6, 128, 128
+    d = dict(batches=2, rows_per_batch=3, a_row_stride=128, a_batch_stride=400, K=K, in_type=2, act=R.ACT_NONE,
+             out_m1=1, out_s0=N)
+    bufs = dict(a=np.ones(400 + 2 * 128 + K, np.int8), w=np.ones((N, K), np.int8), bias=np.zeros(N, np.float32),
+                col_scale=np.ones(N, np.float32), row_scale=np.ones(rows, np.float32), out=np.zeros(rows * N, np.float16))
     return d, bufs
 
 
 def _call(d, bufs, short=None):
-    """b200_test_gemm_desc on the buffers, K = 64 and N = 128, each length as given except `short`'s, one less."""
+    """b200_test_gemm_desc on the buffers, N = 128 and K = 64 unless d sets it, each length as given except `short`'s,
+    one less."""
     import ctypes as C
     from dorado_b200 import lib as L
     t = L.GemmTestDesc()
-    ss = np.zeros(6 * 4, np.float32)
-    for name, arr in dict(bufs, out_ss=ss).items():
+    for name, arr in bufs.items():
         setattr(t, name, arr.ctypes.data)
         setattr(t, name + "_len", arr.size - (name == short))
     t.K, t.N, t.norm_eps = 64, 128, 1e-5
@@ -174,16 +186,88 @@ def _status(fn):
     return L.B200_OK, ""
 
 
-@pytest.mark.parametrize("buf", ["a", "w", "bias", "residual", "res_gain", "a_ss", "res_ss", "out", "out_ss"])
+@pytest.mark.parametrize("buf", ["a", "w", "bias", "residual", "res_gain", "a_ss", "res_ss", "out", "out_ss", "col_scale",
+                                 "row_scale"])
 def test_hook_refuses_short_buffers(buf):
     """One element short of what the descriptor reaches: B200_ERR_INVALID, naming the buffer, before any device work.
     At the exact length the hook goes on (to the device check here, to the GEMM on a GPU)."""
     from dorado_b200 import lib as L
-    d, bufs = _hook_case()
+    d, bufs = _hook_case_s8() if buf in ("col_scale", "row_scale") else _hook_case()
     status, _ = _status(lambda: _call(d, bufs))
     assert status != L.B200_ERR_INVALID
     status, msg = _status(lambda: _call(d, bufs, short=buf))
     assert status == L.B200_ERR_INVALID and f"{buf} is too short" in msg.lower(), (buf, status, msg)
+
+
+# gemm.cu's table of kernel forms: (A and W type, output type, activation, row factors) -> the optional inputs the form
+# reads.  GemmType 0 fp16, 1 E4M3, 2 int8; col_scale is required where it is read.
+F16, E4M3, S8 = 0, 1, 2
+PLAIN = {"bias", "residual", "a_ss", "out_ss"}
+FORMS = {
+    **{(F16, F16, act, False): PLAIN for act in (R.ACT_NONE, R.ACT_SWISH, R.ACT_SWISH_CLAMP, R.ACT_TANH, R.ACT_TANH_X5)},
+    (F16, F16, R.ACT_SWIGLU, False): {"bias", "a_ss"},
+    (F16, F16, R.ACT_ROPE, False): {"a_ss"},
+    (F16, S8, R.ACT_TANH, False): {"bias"},
+    (E4M3, F16, R.ACT_NONE, False): PLAIN,
+    (E4M3, E4M3, R.ACT_SWIGLU, False): {"bias", "a_ss"},
+    (S8, F16, R.ACT_NONE, False): {"col_scale", "bias"},
+    (S8, F16, R.ACT_TANH_X5, False): {"col_scale", "bias"},
+    (S8, F16, R.ACT_NONE, True): {"col_scale", "bias"},
+    (S8, F16, R.ACT_ROPE, True): {"col_scale"},
+}
+OPTIONAL = ("bias", "residual", "a_ss", "out_ss", "col_scale")
+
+
+def _form_call(key, given):
+    """b200_test_gemm_desc on 4 rows, K = N = 128, with the types, activation and row factors of `key` and the optional
+    inputs named in `given`: buffers valid for every form, so that on a GPU an accepted form just runs."""
+    from dorado_b200 import lib as L
+    in_type, out_type, act, rows = key
+    M, K, N = 4, 128, 128
+    n_out = N // 2 if act == R.ACT_SWIGLU else N
+    inputs = dict(bias=np.zeros(N, np.float32), residual=np.zeros(M * N, np.float16), a_ss=np.ones(M, np.float32),
+                  col_scale=np.ones(N, np.float32))
+    kw = {k: v for k, v in inputs.items() if k in given}
+    if "residual" in given:
+        kw.update(alpha=1.0)
+    if "a_ss" in given:
+        kw.update(a_ss_parts=1, norm_dim=K)
+    if act == R.ACT_ROPE:
+        kw.update(theta=1e4, max_seq_len=8, rope_T=4, rope_cols=N)
+    dt = L.GEMM_DTYPES
+    L.test_gemm_desc(np.zeros(M * K, dt[in_type]), np.zeros((N, K), dt[in_type]), np.zeros(M * n_out, dt[out_type]),
+                     rows_per_batch=M, a_row_stride=K, out_s0=n_out, act=act, in_type=in_type, out_type=out_type,
+                     row_scale=np.ones(M, np.float32) if rows else None, out_ss="out_ss" in given, **kw)
+
+
+def test_hook_accepts_exactly_the_kernel_forms():
+    """Every (A and W type, output type, activation, row factors): exactly the table's 14 get past the form check (to the
+    device check here, to the GEMM on a GPU); every other one is refused before any device work."""
+    from dorado_b200 import lib as L
+    acts = (R.ACT_NONE, R.ACT_SWISH, R.ACT_SWISH_CLAMP, R.ACT_TANH, R.ACT_TANH_X5, R.ACT_SWIGLU, R.ACT_ROPE)
+    accepted = set()
+    for key in itertools.product((F16, E4M3, S8), (F16, E4M3, S8), acts, (False, True)):
+        status, msg = _status(lambda: _form_call(key, {"col_scale"} if key[0] == S8 else set()))
+        if status != L.B200_ERR_INVALID:
+            accepted.add(key)
+        else:
+            assert "no kernel form" in msg, (key, msg)
+    assert accepted == set(FORMS)
+
+
+@pytest.mark.parametrize("key", list(FORMS), ids=str)
+def test_hook_takes_the_inputs_each_form_reads(key):
+    """Each optional input, added to (or, for the required col_scale, taken from) the form's required inputs: accepted
+    exactly where the form reads it, and refused, naming it, before any device work where it does not."""
+    from dorado_b200 import lib as L
+    reads = FORMS[key]
+    required = reads & {"col_scale"}
+    for name in OPTIONAL:
+        status, msg = _status(lambda: _form_call(key, required ^ {name}))
+        if name in reads and name not in required:
+            assert status != L.B200_ERR_INVALID, (key, name, msg)
+        else:
+            assert status == L.B200_ERR_INVALID and name in msg, (key, name, status, msg)
 
 
 def test_hook_refuses_bad_addressing():

@@ -183,13 +183,15 @@ def _entries(log, pattern):
     return out
 
 
-def test_ptxas_reports_no_spills_in_the_int8_kernels():
+def test_ptxas_reports_no_spills_in_the_int8_kernel_forms():
     """The int8 instantiations: no stack, no spills, within the registers one CTA per SM of their block size allows."""
     if not (BUILD / "gemm.ptxas.log").is_file() or not (BUILD / "lstm_model.ptxas.log").is_file():
         pytest.skip("the ptxas logs are not built")
-    gemm = _entries("gemm.ptxas.log", r"gemm_wgmma_kernelILi(n?\d+)ELb([01])ELi([12])EE")
-    # (activation, fp8, q8): int8 operands with the plain and tanh x 5 epilogues, fp16 operands with the int8 tanh store
-    assert sorted(gemm) == [("2", "0", "2"), ("3", "0", "1"), ("n1", "0", "1")]
+    forms = _entries("gemm.ptxas.log", r"gemm_wgmma_kernelILi(n?\d+)ELNS_8GemmTypeE(\d)ELS\d+_(\d)ELb([01])EE")
+    # (activation, operand type, output type, row factors), GemmType 0 fp16, 2 int8: int8 operands with the plain and
+    # tanh x 5 epilogues, fp16 operands with the int8 tanh store
+    gemm = {k: v for k, v in forms.items() if (k[1] == "2" and k[3] == "0") or k[2] == "2"}
+    assert sorted(gemm) == [("2", "0", "2", "0"), ("3", "2", "0", "0"), ("n1", "2", "0", "0")]
     for key, (regs, stack, st, ld) in gemm.items():
         print(f"\n[gemm_wgmma_kernel<{key}>] {regs} registers, {stack} B stack, {st} / {ld} B spills")
         assert stack == 0 and st == 0 and ld == 0 and regs * 384 <= 65536

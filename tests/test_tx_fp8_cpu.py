@@ -166,7 +166,7 @@ def _ptxas_entries():
     out = {}
     for block in re.split(r"ptxas info\s*: Compiling entry function ", text)[1:]:
         name = block.split("'")[1]
-        m = re.search(r"gemm_wgmma_kernelILi(n?\d+)ELb([01])E", name)
+        m = re.search(r"gemm_wgmma_kernelILi(n?\d+)ELNS_8GemmTypeE(\d)E", name)   # activation, operand type
         if not m:
             continue
         frame = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", block)
@@ -175,7 +175,7 @@ def _ptxas_entries():
     return out
 
 
-def test_ptxas_reports_no_spills():
+def test_ptxas_reports_no_spills_in_the_e4m3_forms():
     """The E4M3 instantiations (plain and SwiGLU epilogues; one kernel serves sup's and tx1536's shapes, the shapes are
     run-time parameters): no stack, no spills, and within the 168 registers one 384-thread CTA per SM allows."""
     if not PTXAS_LOG.is_file():

@@ -1,4 +1,4 @@
-"""The fp8_ffn transformer precision on the GPU: the E4M3 GEMM alone (b200_test_gemm_fp8) against float64 products of the
+"""The fp8_ffn transformer precision on the GPU: the E4M3 GEMM alone (lib.test_gemm_fp8) against float64 products of the
 decoded operands, sup and tx1536 scores against the FP8-emulating oracle (tests/tx_fp8_ref.py), calls against the C decoder
 oracle, FP8 against fp16 on the same batch, the default precision against an explicit fp16, independence of the runner
 count and batch shape, and the error paths.  The CPU side is tests/test_tx_fp8_cpu.py."""

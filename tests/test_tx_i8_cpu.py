@@ -278,15 +278,15 @@ def _ptxas(log, pattern):
     return out
 
 
-def test_ptxas_reports_no_spills():
-    """The GEMM's int8 instantiations with row factors (template Q8 = 3: the RoPE and the plain epilogue), the quantise
+def test_ptxas_reports_no_spills_in_the_row_factor_forms():
+    """The GEMM's int8 instantiations with row factors (template ROWS: the RoPE and the plain epilogue), the quantise
     kernel and rmsnorm_kernel with its int8 form: no stack, no spills, and the GEMMs within the 168 registers one 384-thread
     CTA per SM allows."""
     if not (BUILD / "gemm.ptxas.log").is_file() or not (BUILD / "tx_model.ptxas.log").is_file():
         pytest.skip("the ptxas logs are not built")
-    gemm = _ptxas("gemm.ptxas.log", r"(gemm_wgmma_kernelIL\w+ELb0ELi3EE)")
+    gemm = _ptxas("gemm.ptxas.log", r"(gemm_wgmma_kernelIL\w+ELb1EE)")
     tx = _ptxas("tx_model.ptxas.log", r"(quantize_i8_kernel|rmsnorm_kernel)")
-    assert set(gemm) == {"gemm_wgmma_kernelILi5ELb0ELi3EE", "gemm_wgmma_kernelILin1ELb0ELi3EE"}
+    assert set(gemm) == {"gemm_wgmma_kernelILi5ELNS_8GemmTypeE2ELS2_0ELb1EE", "gemm_wgmma_kernelILin1ELNS_8GemmTypeE2ELS2_0ELb1EE"}
     assert set(tx) == {"quantize_i8_kernel", "rmsnorm_kernel"}
     for name, (regs, stack, st, ld) in {**gemm, **tx}.items():
         print(f"\n[{name}] {regs} registers, {stack} B stack, {st} / {ld} B spills")

@@ -1,5 +1,5 @@
 """The int8_qkv_fp8_ffn transformer precision on the GPU: the device quantiser (b200_test_quantize_act_rows) against the host
-quantize_rows_f16 bit for bit, the s8 GEMM with row and column factors (b200_test_gemm_s8_scaled) against float64, every
+quantize_rows_f16 bit for bit, the s8 GEMM with row and column factors (lib.test_gemm_s8_scaled) against float64, every
 launch of the plan against tests/tx_i8_ref.py's per-launch reference from the engine's own buffers, sup and tx1536 scores
 against the int8 restatement, calls against the C decoder oracle, and the interface.  The CPU side is
 tests/test_tx_i8_cpu.py.  Measured worst cases: DESIGN.md section 2."""
